@@ -157,9 +157,9 @@ int nrc_eval_force_exact(int32_t on);
 /* How many users of the last nrc_eval_mf / nrc_eval_mf_tc call needed a heap replay (host int32 out). */
 int nrc_eval_last_undecided(int32_t* count_host);
 
-/* nrc_eval_mf for large catalogues (BASELINE config 4) with the score step on the 5th-gen
- * tensor cores: bf16 copies of the tables, wgmma (64 users x 128 items x k16 per warpgroup) with fp32
- * accumulators, a per-user running threshold (the 2*top_k-th best score so far,
+/* nrc_eval_mf for large catalogues (BASELINE config 4) with the score step on the Hopper tensor
+ * cores: bf16 copies of the tables, wgmma (64 users x 128 items x k16 per warpgroup, 64 items at
+ * dim 192) with fp32 accumulators, a per-user running threshold (the 2*top_k-th best score so far,
  * the reference's heap root, evaluate.h:38-41) with a rigorous error margin to keep every item
  * that can enter the reference's heap, then exact fp32 re-scoring of the candidates, the same
  * tie-aware selection as nrc_eval_mf and -- for users with ties -- the libstdc++ heap replayed
@@ -191,9 +191,34 @@ int nrc_eval_tc_last_launch(float* kernel_ms, double* flops);
 
 /* Self-test of the wgmma building block used by the tensor-core candidate pass:
  * out f32 [128, 256] = a bf16 [128, k] . b bf16 [256, k]^T (k multiple of 16, <= 256);
- * swizzle = 0: no-swizzle K-major operand layout, 1: SWIZZLE_128B (k % 64 == 0). */
+ * swizzle = 0: no-swizzle K-major operand layout, 1: SWIZZLE_128B (k % 64 == 0).
+ * nrc_tc_gemm_debug issues wgmma m64n128k16 (the instruction of dim <= 128); nrc_tc_gemm_debug_ntile
+ * takes the N tile: n_tile = 128 (m64n128k16) or 64 (m64n64k16, the instruction of dim 192). */
 int nrc_tc_gemm_debug(const void* a_bf16, const void* b_bf16, int32_t k, int32_t swizzle, float* out,
                       void* stream);
+int nrc_tc_gemm_debug_ntile(const void* a_bf16, const void* b_bf16, int32_t k, int32_t swizzle, int32_t n_tile,
+                            float* out, void* stream);
+
+/* Test hooks of the tensor-core path (all off by default; they change no result).
+ * nrc_eval_tc_force_segments: g = 0 keeps the occupancy heuristic for the number of item segments
+ *   (lists per user) of both candidate passes; g >= 1 uses min(g, item tiles) segments.
+ * nrc_eval_tc_debug_candidates: runs ONE candidate pass (pass 0: main, 1: tie replay) exactly as
+ *   nrc_eval_mf_tc would -- bf16 tables, margin, forced or heuristic segments, 16-warp epilogue
+ *   (nrc_eval_tc_epilogue_warps) in pass 0 only -- with threshold rank lq and cap entries per list,
+ *   and copies out cand i32 / cand_val f32 (approximate score) [n, nslots, cap], cnt i32 [n, nslots]
+ *   (> cap: the list overflowed) and margin f32 [n] into device buffers sized for max_slots lists per
+ *   row.  *nslots and *seg_items (items per segment) are HOST outputs; NRC_E_LIMIT when the pass uses
+ *   more than max_slots lists.
+ * nrc_eval_tc_last_fallbacks: users of the last nrc_eval_mf_tc call re-ranked by the candidate-list
+ *   heap replay (ties) and by the full-catalogue heap replay (an overflowed list); HOST outputs,
+ *   synchronises the device. */
+int nrc_eval_tc_force_segments(int32_t g);
+int nrc_eval_tc_debug_candidates(int32_t pass, const float* user_table, const float* item_table, int32_t dim,
+                                 int32_t num_items, const int32_t* users, int32_t n, const int64_t* train_indptr,
+                                 const int32_t* train_indices, int32_t lq, int32_t cap, int32_t max_slots,
+                                 int32_t* cand, float* cand_val, int32_t* cnt, float* margin, int32_t* nslots,
+                                 int32_t* seg_items, void* stream);
+int nrc_eval_tc_last_fallbacks(int32_t* replayed, int32_t* full_replays);
 
 /* MF.predict(user_ids, None), model/general_recommender/MF.py:120-122 (np.matmul(U[users], V.T))
  * and LightGCN.predict, LightGCN.py:187-189, materialised: scores f32 [num_rows, num_items]

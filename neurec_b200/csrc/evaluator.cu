@@ -937,6 +937,18 @@ extern "C" int nrc_eval_last_undecided(int32_t* count_host) {
     return NRC_OK;
 }
 
+// Routes of the last nrc_eval_mf_tc call: users re-ranked by the candidate-list heap replay (ties) and users
+// re-ranked by the full-catalogue eval_mf_kernel (an overflowed candidate list in either pass).  The second
+// count lives on the device, so this synchronises.
+extern "C" int nrc_eval_tc_last_fallbacks(int32_t* replayed, int32_t* full_replays) {
+    NRC_REQUIRE(replayed != nullptr && full_replays != nullptr, NRC_E_VALUE, "NULL output");
+    NRC_REQUIRE(g_last_was_tc && g_slow != nullptr, NRC_E_VALUE, "the last evaluation was not nrc_eval_mf_tc");
+    *replayed = g_last_replays;
+    NRC_CUDA_CHECK(cudaDeviceSynchronize());   // whatever stream the call ran on
+    NRC_CUDA_CHECK(cudaMemcpy(full_replays, g_slow, sizeof(int32_t), cudaMemcpyDeviceToHost));
+    return NRC_OK;
+}
+
 extern "C" int nrc_eval_mf(const float* user_table, const float* item_table, int32_t dim,
                            int32_t num_items, const int32_t* users, int32_t num_eval_users,
                            const int64_t* train_indptr, const int32_t* train_indices,

@@ -151,10 +151,12 @@ __device__ __forceinline__ uint64_t kmajor_desc(uint32_t tile_base, int rows, in
 
 // ----------------------------------------------------------------------------------------
 // Self-test kernel: out[128, 256] = A[128, K] . B[256, K]^T through wgmma.  Two warpgroups, 64
-// rows of A each, two m64n128 halves of B.
+// rows of A each, 256 / NT m64nNTk16 column blocks of B (NT = 128 or 64, the two instructions the
+// candidate kernel issues).
 // ----------------------------------------------------------------------------------------
 constexpr int kDbgM = 128, kDbgN = 256;
 
+template <int NT>
 __global__ void __launch_bounds__(256)
 tc_gemm_debug_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* __restrict__ B, int K,
                      float* __restrict__ out, int swizzle) {
@@ -173,23 +175,24 @@ tc_gemm_debug_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* _
     fence_async_smem();
     __syncthreads();
     const uint32_t a0 = smem_u32(sA), b0 = smem_u32(sB);
-    for (int nh = 0; nh < 2; ++nh) {
-        float d[64];
+    for (int nh = 0; nh < kDbgN / NT; ++nh) {
+        float d[NT / 2];
 #pragma unroll
-        for (int i = 0; i < 64; ++i) d[i] = 0.0f;
+        for (int i = 0; i < NT / 2; ++i) d[i] = 0.0f;
         wgmma_fence();
         for (int s = 0; s < K / kMmaK; ++s) {
             const uint64_t ad = swizzle ? sw128_desc(a0, kDbgM, wg * kWgM, s) : kmajor_desc(a0, kDbgM, wg * kWgM, s);
-            const uint64_t bd = swizzle ? sw128_desc(b0, kDbgN, nh * 128, s) : kmajor_desc(b0, kDbgN, nh * 128, s);
-            wgmma_m64n128k16(d, ad, bd, s > 0 ? 1u : 0u);
+            const uint64_t bd = swizzle ? sw128_desc(b0, kDbgN, nh * NT, s) : kmajor_desc(b0, kDbgN, nh * NT, s);
+            if constexpr (NT == 128) wgmma_m64n128k16(d, ad, bd, s > 0 ? 1u : 0u);
+            else wgmma_m64n64k16(d, ad, bd, s > 0 ? 1u : 0u);
         }
         wgmma_commit();
         wgmma_wait_all();
         wgmma_keep(d);
         const int r0 = wg * kWgM + 16 * (t >> 5) + ((t & 31) >> 2);
 #pragma unroll
-        for (int i = 0; i < 64; ++i) {
-            const int row = r0 + 8 * ((i >> 1) & 1), col = nh * 128 + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
+        for (int i = 0; i < NT / 2; ++i) {
+            const int row = r0 + 8 * ((i >> 1) & 1), col = nh * NT + 8 * (i >> 2) + 2 * (t & 3) + (i & 1);
             out[(size_t)row * kDbgN + col] = d[i];
         }
     }
@@ -200,19 +203,26 @@ tc_gemm_debug_kernel(const __nv_bfloat16* __restrict__ A, const __nv_bfloat16* _
 
 using namespace nrc;
 
-// Test hook: out f32 [128, 256] = A bf16 [128, K] . B bf16 [256, K]^T  (K multiple of 16, <= 256).
-extern "C" int nrc_tc_gemm_debug(const void* a_bf16, const void* b_bf16, int32_t k, int32_t swizzle, float* out,
-                                 void* stream) {
+// Test hook: out f32 [128, 256] = A bf16 [128, K] . B bf16 [256, K]^T  (K multiple of 16, <= 256), through
+// wgmma m64n128k16 (n_tile 128) or m64n64k16 (n_tile 64).
+extern "C" int nrc_tc_gemm_debug_ntile(const void* a_bf16, const void* b_bf16, int32_t k, int32_t swizzle,
+                                       int32_t n_tile, float* out, void* stream) {
     NRC_REQUIRE(k >= 16 && k <= 256 && (k % 16) == 0, NRC_E_LIMIT, "k must be a multiple of 16 in [16, 256]");
     NRC_REQUIRE(!swizzle || (k % 64) == 0, NRC_E_LIMIT, "the SWIZZLE_128B layout needs k % 64 == 0");
+    NRC_REQUIRE(n_tile == 64 || n_tile == 128, NRC_E_VALUE, "n_tile must be 64 or 128 (got %d)", n_tile);
     const size_t smem = (size_t)(tc::kDbgM + tc::kDbgN) * k * 2 + 1024;
-    NRC_CUDA_CHECK(cudaFuncSetAttribute(tc::tc_gemm_debug_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)smem));
-    tc::tc_gemm_debug_kernel<<<1, 256, smem, as_stream(stream)>>>(
-        reinterpret_cast<const __nv_bfloat16*>(a_bf16), reinterpret_cast<const __nv_bfloat16*>(b_bf16), k, out,
-        swizzle);
+    auto kern = n_tile == 128 ? tc::tc_gemm_debug_kernel<128> : tc::tc_gemm_debug_kernel<64>;
+    NRC_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<1, 256, smem, as_stream(stream)>>>(reinterpret_cast<const __nv_bfloat16*>(a_bf16),
+                                              reinterpret_cast<const __nv_bfloat16*>(b_bf16), k, out, swizzle);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
+}
+
+// The same with the m64n128k16 instruction (the original signature, kept for its callers).
+extern "C" int nrc_tc_gemm_debug(const void* a_bf16, const void* b_bf16, int32_t k, int32_t swizzle, float* out,
+                                 void* stream) {
+    return nrc_tc_gemm_debug_ntile(a_bf16, b_bf16, k, swizzle, 128, out, stream);
 }
 
 // =========================================================================================
@@ -476,6 +486,8 @@ __global__ void tc_prepare_items_kernel(const float* __restrict__ V, int64_t N, 
 //   adder, d <= 192 terms) and the fp32 FMA chain of the exact score add < 2^-11 |u| |v| together.
 //   eps = (2^-7 + 2^-11) * |u| * max_i |v_i| * 1.001 (norms are fp32-rounded), margin = 2 * eps:
 //   an item's approximate score and the order statistic it is compared with each move by <= eps.
+//   The wgmma accumulation term is measured by tests/test_gpu_tc_eval.py (adversarial k = 256 operands:
+//   <= 2^-20 sum|u_k v_k|), and subnormal products by tests/test_gpu_tc_candidates.py (within eps).
 __global__ void tc_prepare_users_kernel(const float* __restrict__ U, const int32_t* __restrict__ users, int num_eval,
                                         int D, const unsigned int* __restrict__ vmax_bits,
                                         __nv_bfloat16* __restrict__ Ub, float* __restrict__ margin) {
@@ -531,6 +543,7 @@ static size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
 // not changed: nrc_eval_tc_items_version(v != 0) keys the cache on (pointer, shape, v); version 0
 // (default) converts on every call.
 static int g_ch_pref = -1;      // filter threads per user: 1 (default) or 2 (nrc_eval_tc_epilogue_warps / NRC_TC_CH)
+static int g_force_segments = 0;   // item segments per pass: 0 = heuristic, g >= 1 = min(g, tiles) (nrc_eval_tc_force_segments)
 static uint64_t g_items_version = 0, g_cached_version = 0;
 static const float* g_cached_ptr = nullptr;
 
@@ -588,6 +601,7 @@ int run_pass(int pass, const float* U, const int32_t* users, int num_rows, const
             if (cost < best - 1e-9) { best = cost; G = g; }
         }
     }
+    if (g_force_segments > 0) G = g_force_segments < T ? g_force_segments : T;   // test hook
     const int seg_tiles = (T + G - 1) / G;
     G = (T + seg_tiles - 1) / seg_tiles;           // no empty segment
     const int nslots = G * CH;
@@ -672,6 +686,7 @@ int run_pass(int pass, const float* U, const int32_t* users, int num_rows, const
     out->cnt = cnt;
     out->nslots = nslots;
     out->cap = cap;
+    out->seg_items = seg_tiles * kNT;
     return NRC_OK;
 }
 
@@ -691,6 +706,44 @@ extern "C" int nrc_eval_tc_items_version(uint64_t version) {
 extern "C" int nrc_eval_tc_epilogue_warps(int32_t warps) {
     NRC_REQUIRE(warps == 8 || warps == 16, NRC_E_VALUE, "epilogue warps must be 8 or 16 (got %d)", warps);
     nrc::tc::g_ch_pref = warps / 8;
+    return NRC_OK;
+}
+
+// Test hook: item segments (grid.y) of both candidate passes.  0 = the occupancy heuristic of run_pass;
+// g >= 1 = min(g, item tiles) segments (then the same "no empty segment" recount).
+extern "C" int nrc_eval_tc_force_segments(int32_t g) {
+    NRC_REQUIRE(g >= 0, NRC_E_VALUE, "segment count must be >= 0 (got %d)", g);
+    nrc::tc::g_force_segments = g;
+    return NRC_OK;
+}
+
+// Test hook: one candidate pass exactly as nrc_eval_mf_tc runs it (prepare_items + run_pass: the same CH rule,
+// the same forced or heuristic segment count), with the lists copied out.  cand / cand_val [n, nslots, cap],
+// cnt [n, nslots], margin [n] are device buffers sized for max_slots lists per row; *nslots and *seg_items
+// are host outputs.
+extern "C" int nrc_eval_tc_debug_candidates(int32_t pass, const float* user_table, const float* item_table,
+                                            int32_t dim, int32_t num_items, const int32_t* users, int32_t n,
+                                            const int64_t* train_indptr, const int32_t* train_indices, int32_t lq,
+                                            int32_t cap, int32_t max_slots, int32_t* cand, float* cand_val,
+                                            int32_t* cnt, float* margin, int32_t* nslots, int32_t* seg_items,
+                                            void* stream) {
+    NRC_REQUIRE(nslots != nullptr && seg_items != nullptr, NRC_E_VALUE, "NULL output");
+    NRC_REQUIRE(n > 0 && cap > 0 && num_items > 0, NRC_E_VALUE, "bad shape");
+    cudaStream_t st = as_stream(stream);
+    int rc = nrc::tc::prepare_items(item_table, dim, num_items, st);
+    if (rc) return rc;
+    nrc::tc::CandLists c;
+    rc = nrc::tc::run_pass(pass, user_table, users, n, train_indptr, train_indices, lq, cap, &c, st);
+    if (rc) return rc;
+    *nslots = c.nslots;
+    *seg_items = c.seg_items;
+    NRC_REQUIRE(c.nslots <= max_slots, NRC_E_LIMIT, "the pass uses %d lists per row (> max_slots %d)", c.nslots,
+                max_slots);
+    const size_t lists = (size_t)n * c.nslots;
+    NRC_CUDA_CHECK(cudaMemcpyAsync(cand, c.cand, lists * cap * 4, cudaMemcpyDeviceToDevice, st));
+    NRC_CUDA_CHECK(cudaMemcpyAsync(cand_val, c.scratch, lists * cap * 4, cudaMemcpyDeviceToDevice, st));
+    NRC_CUDA_CHECK(cudaMemcpyAsync(cnt, c.cnt, lists * 4, cudaMemcpyDeviceToDevice, st));
+    NRC_CUDA_CHECK(cudaMemcpyAsync(margin, c.margin, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
     return NRC_OK;
 }
 

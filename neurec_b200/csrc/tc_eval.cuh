@@ -13,6 +13,7 @@ struct CandLists {
                            // them with exact ones)
     const float* margin;   // [rows] the per-user error margin the candidate kernel used
     int nslots, cap;
+    int seg_items;         // items per segment: list s covers items [(s / CH) * seg_items, ...)
 };
 
 // bf16 copy of the item table + its largest row norm, kept in a library-owned buffer until the

@@ -206,6 +206,56 @@ def eval_tc_last_launch():
     return ms.value, fl.value
 
 
+def eval_tc_force_segments(g):
+    """Test hook: 0 = heuristic number of item segments in the tensor-core passes, g >= 1 = min(g, tiles)."""
+    check(_lib.load().nrc_eval_tc_force_segments(int(g)))
+
+
+def eval_tc_debug_candidates(pass_, user_table, item_table, users, train_indptr, train_indices, lq, cap, max_slots):
+    """Test hook: one tensor-core candidate pass as eval_mf_tc runs it.  Returns (cand [n, nslots, cap] int32,
+    cand_val [n, nslots, cap] float32 approximate scores, cnt [n, nslots] int32 (> cap: overflow), margin [n]
+    float32, seg_items); entries of a list past min(cnt, cap) are undefined."""
+    _req(user_table, torch.float32, "user_table")
+    _req(item_table, torch.float32, "item_table")
+    _req(users, torch.int32, "users")
+    N, D = item_table.shape
+    n = users.numel()
+    dev = users.device
+    cand = torch.empty((n * max_slots * cap,), dtype=torch.int32, device=dev)
+    val = torch.empty((n * max_slots * cap,), dtype=torch.float32, device=dev)
+    cnt = torch.empty((n * max_slots,), dtype=torch.int32, device=dev)
+    margin = torch.empty((n,), dtype=torch.float32, device=dev)
+    ns, seg = ctypes.c_int32(0), ctypes.c_int32(0)
+    check(_lib.load().nrc_eval_tc_debug_candidates(
+        int(pass_), _p(user_table), _p(item_table), D, N, _p(users), n, _p(train_indptr), _p(train_indices),
+        int(lq), int(cap), int(max_slots), _p(cand), _p(val), _p(cnt), _p(margin), ctypes.byref(ns),
+        ctypes.byref(seg), _stream()))
+    _count(3)
+    s = ns.value
+    return (cand[:n * s * cap].view(n, s, cap), val[:n * s * cap].view(n, s, cap), cnt[:n * s].view(n, s),
+            margin, seg.value)
+
+
+def eval_tc_last_fallbacks():
+    """(users of the last eval_mf_tc call re-ranked by the candidate-list heap replay, users re-ranked by the
+    full-catalogue heap replay after a candidate list overflowed)."""
+    r, f = ctypes.c_int32(0), ctypes.c_int32(0)
+    check(_lib.load().nrc_eval_tc_last_fallbacks(ctypes.byref(r), ctypes.byref(f)))
+    return r.value, f.value
+
+
+def tc_gemm_debug(a, b, swizzle=1, n_tile=128):
+    """Test hook: out f32 [128, 256] = a bf16 [128, k] . b bf16 [256, k]^T through wgmma m64n{n_tile}k16."""
+    _req(a, torch.bfloat16, "a")
+    _req(b, torch.bfloat16, "b")
+    assert a.shape[0] == 128 and b.shape[0] == 256 and a.shape[1] == b.shape[1]
+    out = torch.empty((128, 256), dtype=torch.float32, device=a.device)
+    check(_lib.load().nrc_tc_gemm_debug_ntile(_p(a), _p(b), a.shape[1], int(swizzle), int(n_tile), _p(out),
+                                              _stream()))
+    _count()
+    return out
+
+
 def eval_last_undecided():
     """Users of the last eval_mf / eval_mf_tc call that needed a heap replay (ties, overflow)."""
     import ctypes

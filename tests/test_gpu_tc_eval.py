@@ -34,6 +34,67 @@ def test_tcgen05_gemm_building_block(K, sw):
     assert (out.double() - ref).abs().max().item() < 2e-4
 
 
+@pytest.mark.parametrize("n_tile", [128, 64])
+@pytest.mark.parametrize("K,sw", [(64, 0), (128, 0), (64, 1), (128, 1), (256, 1)])
+def test_wgmma_gemm_building_block_both_n_tiles(K, sw, n_tile):
+    """nrc_tc_gemm_debug_ntile: the wgmma building block with either instruction the candidate kernel issues,
+    m64n128k16 (dim <= 128) and m64n64k16 (dim 192), both operand layouts."""
+    from neurec_b200 import ops
+    g = torch.Generator(device="cuda").manual_seed(K + sw)
+    A = torch.randn(128, K, device="cuda", generator=g).bfloat16()
+    B = torch.randn(256, K, device="cuda", generator=g).bfloat16()
+    out = ops.tc_gemm_debug(A, B, swizzle=sw, n_tile=n_tile)
+    torch.cuda.synchronize()
+    ref = A.double() @ B.double().T          # bf16 products are exact; only the fp32 accumulation differs
+    assert (out.double() - ref).abs().max().item() < 2e-4
+
+
+def _accumulation_operands(pattern, k, rs):
+    """bf16-exact operands A [128, k], B [256, k] whose fp32 accumulation is hard to get right."""
+    if pattern == "unit_plus_tiny":
+        # per k16 block: one product of size ~1 and fifteen just under 2^-24 of it, all of one sign per
+        # dot product; the unit product sits at a row- / column-dependent position of the block
+        A = np.full((128, k), 2.0 ** -12 * (1 - 2.0 ** -8))
+        B = np.full((256, k), 2.0 ** -12)
+        pa, pb = rs.randint(0, 16, 128), rs.randint(0, 16, 256)
+        pb[:128] = pa                                          # half of the pairs: the designed pattern exactly
+        for b in range(k // 16):
+            A[np.arange(128), 16 * b + pa] = 1.0
+            B[np.arange(256), 16 * b + pb] = 1.0
+        A *= rs.choice([-1.0, 1.0], (128, 1)) * 2.0 ** rs.randint(-20, 20, (128, 1))
+        B *= 2.0 ** rs.randint(-20, 20, (256, 1))
+    elif pattern == "cancelling":
+        # +-x pairs: the products cancel up to small residues
+        x = 2.0 ** rs.randint(-6, 6, (128, k // 2)) * (1 + rs.randint(0, 128, (128, k // 2)) / 128.0)
+        A = np.repeat(x, 2, axis=1)
+        y = 2.0 ** rs.randint(-6, 6, (256, k // 2)) * (1 + rs.randint(0, 128, (256, k // 2)) / 128.0)
+        B = np.repeat(y, 2, axis=1)
+        B[:, 1::2] *= -(1 - rs.randint(0, 3, (256, k // 2)) * 2.0 ** -7)
+    else:
+        A, B = rs.randn(128, k), rs.randn(256, k)
+    return torch.tensor(A, dtype=torch.float32).bfloat16(), torch.tensor(B, dtype=torch.float32).bfloat16()
+
+
+@pytest.mark.parametrize("sw", [0, 1])
+@pytest.mark.parametrize("n_tile", [128, 64])
+def test_wgmma_accumulation_error_within_half_the_margin_budget(n_tile, sw):
+    """The margin (tc_prepare_users_kernel) leaves 2^-11 |u||v| for the tensor core's fp32 accumulation and
+    the exact FMA chain together.  Measured on adversarial operands at k = 256: |out - sum bf16(a) bf16(b)
+    (fp64)| must stay below 2^-12 sum |a_k b_k|, half of that budget."""
+    from neurec_b200 import ops
+    rs = np.random.RandomState(n_tile + sw)
+    worst = 0.0
+    for pattern in ("unit_plus_tiny", "cancelling", "gauss"):
+        A, B = _accumulation_operands(pattern, 256, rs)
+        out = ops.tc_gemm_debug(A.cuda(), B.cuda(), swizzle=sw, n_tile=n_tile).cpu().double()
+        a, b = A.double(), B.double()
+        ref, mag = a @ b.T, a.abs() @ b.abs().T
+        err = (out - ref).abs()
+        assert (err <= 2.0 ** -12 * mag).all(), (pattern, float((err / mag.clamp_min(1e-300)).max()))
+        worst = max(worst, float((err / mag.clamp_min(1e-300)).max()) / 2.0 ** -12)
+    print("n_tile %d swizzle %d: largest |error| / (2^-12 sum|ab|) = %.3g" % (n_tile, sw, worst))
+
+
 def _problem(nu, ni, dim, seed, scale=0.1, int_tables=False):
     rs = np.random.RandomState(seed)
     if int_tables:
@@ -201,3 +262,184 @@ def test_tc_eval_sixteen_epilogue_warps_give_the_same_bits():
             assert np.array_equal(got.cpu().numpy(), want)
     finally:
         ops.eval_tc_epilogue_warps(8)
+
+
+def _force_exact(on):
+    from neurec_b200 import _lib
+    _lib.check(_lib.load().nrc_eval_force_exact(int(on)))
+
+
+@pytest.mark.parametrize("dim,ni,K", [(64, 20049, 20), (192, 20001, 12)])
+def test_tc_eval_forced_segments_bit_exact(dim, ni, K):
+    """The replay pass over G > 1 item segments (lists replayed in slot order) on integer tables (mass ties),
+    with and without the tie-free main pass: ranks and metric rows equal the oracle's for every G and both
+    epilogue layouts."""
+    from neurec_b200 import ops
+    nu = 130
+    U, V, tp, ti, sp, si = _problem(nu, ni, dim, 41 + dim, int_tables=True)
+    users = np.arange(nu, dtype=np.int32)
+    want, wranks = oracle.eval_mf(U, V, users, tp, ti, sp, si, ALL, K, thread_num=8, return_ranks=True)
+    d = (dev(U), dev(V), dev(users), dev(tp), dev(ti), dev(sp), dev(si))
+    try:
+        for G in (1, 2, 3, 7, 16):
+            ops.eval_tc_force_segments(G)
+            # the route: the replay pass really runs over G lists per user
+            lists = ops.eval_tc_debug_candidates(1, d[0], d[1], d[2][:3], d[3], d[4], min(2 * K, ni), 2048, 64)
+            assert lists[2].shape[1] == G
+            for CH in (1, 2):
+                ops.eval_tc_epilogue_warps(8 * CH)
+                for exact in (1, 0):
+                    _force_exact(exact)
+                    got, ranks = ops.eval_mf_tc(*d, ALL, K, return_ranks=True)
+                    replayed, full = ops.eval_tc_last_fallbacks()
+                    assert np.array_equal(ranks.cpu().numpy(), wranks), (G, CH, exact)
+                    assert np.array_equal(got.cpu().numpy(), want), (G, CH, exact)
+                    assert replayed > 0, (G, CH, exact, replayed, full)
+                    if exact:
+                        assert replayed + full == nu
+    finally:
+        _force_exact(0)
+        ops.eval_tc_force_segments(0)
+        ops.eval_tc_epilogue_warps(8)
+
+
+@pytest.mark.parametrize("G", [2, 3, 7])
+def test_tc_eval_ties_straddling_segment_boundaries(G):
+    """Identical item rows on both sides of every segment boundary: their scores tie at the top, so which of
+    them the reference's heap keeps, and in which order, depends on the order the replay visits its lists."""
+    from neurec_b200 import ops
+    nu, ni, dim, K = 130, 24000, 64, 10
+    rs = np.random.RandomState(G)
+    V = (rs.randn(ni, dim) * 0.1).astype(np.float32)
+    hubs = (rs.randn(3, dim) * 0.4).astype(np.float32)
+    T = -(-ni // 128)
+    seg_items = -(-T // G) * 128
+    for b in range(seg_items, ni, seg_items):
+        for off in (-3, -2, -1, 0, 1, 2):                                  # every hub on both sides
+            V[b + off] = hubs[off % 3]
+    U = (hubs[rs.randint(0, 3, nu)] + rs.randn(nu, dim).astype(np.float32) * 0.02).astype(np.float32)
+    U[::5] = (rs.randn(nu // 5, dim) * 0.1).astype(np.float32)            # and some users without a hub
+    users = np.arange(nu, dtype=np.int32)
+    tp, ti = random_csr(rs, nu, ni, rs.randint(0, 30, nu))
+    sp, si = random_csr(rs, nu, ni, rs.randint(1, 12, nu))
+    want, wranks = oracle.eval_mf(U, V, users, tp, ti, sp, si, ALL, K, thread_num=8, return_ranks=True)
+    d = (dev(U), dev(V), dev(users), dev(tp), dev(ti), dev(sp), dev(si))
+    try:
+        ops.eval_tc_force_segments(G)
+        assert ops.eval_tc_debug_candidates(1, d[0], d[1], d[2], d[3], d[4], 2 * K, 2048, G)[4] == seg_items
+        for exact in (0, 1):
+            _force_exact(exact)
+            got, ranks = ops.eval_mf_tc(*d, ALL, K, return_ranks=True)
+            replayed, full = ops.eval_tc_last_fallbacks()
+            assert replayed > nu // 2 and full == 0, (exact, replayed, full)
+            assert np.array_equal(ranks.cpu().numpy(), wranks), exact
+            assert np.array_equal(got.cpu().numpy(), want), exact
+    finally:
+        _force_exact(0)
+        ops.eval_tc_force_segments(0)
+
+
+def test_tc_eval_replay_pass_overflow_falls_back_to_full_replay():
+    """{0, 1} tables, dim 64, ~50 k items: for half of the users 40 items tie at the top (the main pass keeps
+    few candidates, but the top K+1 tie) and 3 000 more tie just below, so that the replay pass's threshold
+    (the 2K-th best) lets more than 2 048 of them through -- the list overflows and the user is re-ranked
+    by the full-catalogue heap replay (eval_mf_kernel)."""
+    from neurec_b200 import ops
+    nu, ni, dim, K = 70, 50_000, 64, 31
+    rs = np.random.RandomState(9)
+    V = (rs.rand(ni, dim) < 0.5).astype(np.float32)
+    V[:, :3] = 0.0
+    V[:40, :3] = 1.0                                                   # score 3 for the special users
+    two = 40 + rs.permutation(ni - 40)[:3000]
+    for j, i in enumerate(two):                                        # score 2
+        V[i, [c for c in range(3) if c != j % 3]] = 1.0
+    one = np.setdiff1d(np.arange(40, ni), two)
+    V[one, rs.randint(0, 3, len(one))] = 1.0                           # score 1
+    U = (rs.rand(nu, dim) < 0.3).astype(np.float32)
+    special = np.arange(0, nu, 2)
+    U[special] = 0.0
+    U[special, :3] = 1.0
+    users = np.arange(nu, dtype=np.int32)
+    tp, ti = random_csr(rs, nu, ni, rs.randint(0, 6, nu))
+    sp, si = random_csr(rs, nu, ni, rs.randint(1, 12, nu))
+    want, wranks = oracle.eval_mf(U, V, users, tp, ti, sp, si, ALL, K, thread_num=8, return_ranks=True)
+    d = (dev(U), dev(V), dev(users), dev(tp), dev(ti), dev(sp), dev(si))
+    try:
+        ops.eval_tc_force_segments(1)
+        sp_users = dev(special.astype(np.int32))
+        c0 = ops.eval_tc_debug_candidates(0, d[0], d[1], sp_users, d[3], d[4], K + 1, 1024, 1)[2].cpu().numpy()
+        c1 = ops.eval_tc_debug_candidates(1, d[0], d[1], sp_users, d[3], d[4], 2 * K, 2048, 1)[2].cpu().numpy()
+        assert (c0 <= 1024).all() and (c1 > 2048).all(), (c0.max(), c1.min())
+        got, ranks = ops.eval_mf_tc(*d, ALL, K, return_ranks=True)
+        replayed, full = ops.eval_tc_last_fallbacks()
+        assert replayed >= len(special) and full >= len(special), (replayed, full)
+        assert np.array_equal(ranks.cpu().numpy(), wranks)
+        assert np.array_equal(got.cpu().numpy(), want)
+    finally:
+        ops.eval_tc_force_segments(0)
+
+
+def test_tc_eval_bf16_item_cache_versions():
+    """nrc_eval_tc_items_version: user batches of one table version equal one call; an in-place change of the
+    table under a new version, and a different table of the same shape under the same version, are
+    converted again."""
+    from neurec_b200 import ops
+    nu, ni, dim, K = 300, 17_000, 64, 10
+    U, V, tp, ti, sp, si = _problem(nu, ni, dim, 23)
+    users = np.arange(nu, dtype=np.int32)
+    d = [dev(U), dev(V), dev(users), dev(tp), dev(ti), dev(sp), dev(si)]
+
+    def oracle_on(Vh):
+        return oracle.eval_mf(U, Vh, users, tp, ti, sp, si, ALL, K, thread_num=8, return_ranks=True)
+
+    def run(Vd, rows=None):
+        u = d[2] if rows is None else d[2][rows]
+        got, ranks = ops.eval_mf_tc(d[0], Vd, u, d[3], d[4], d[5], d[6], ALL, K, return_ranks=True)
+        return got.cpu().numpy(), ranks.cpu().numpy()
+
+    try:
+        ops.eval_tc_items_version(1)
+        want, wranks = oracle_on(V)
+        got, ranks = run(d[1])
+        assert np.array_equal(ranks, wranks) and np.array_equal(got, want)
+        a, b = run(d[1], slice(0, 150)), run(d[1], slice(150, nu))
+        assert np.array_equal(np.concatenate([a[1], b[1]]), ranks)
+        assert np.array_equal(np.concatenate([a[0], b[0]]), got)
+        # in place, new version: must be converted again
+        V2 = (V[::-1] * np.float32(1.5)).copy()
+        d[1].copy_(dev(V2))
+        ops.eval_tc_items_version(2)
+        want2, wranks2 = oracle_on(V2)
+        got, ranks = run(d[1])
+        assert np.array_equal(ranks, wranks2) and np.array_equal(got, want2)
+        # another table of the same shape under the same version
+        V3 = (np.random.RandomState(5).randn(ni, dim) * 0.1).astype(np.float32)
+        d3 = dev(V3)
+        want3, wranks3 = oracle_on(V3)
+        got, ranks = run(d3)
+        assert np.array_equal(ranks, wranks3) and np.array_equal(got, want3)
+        got, ranks = run(d[1])                                         # and back
+        assert np.array_equal(ranks, wranks2) and np.array_equal(got, want2)
+    finally:
+        ops.eval_tc_items_version(0)
+
+
+@pytest.mark.parametrize("dim", [64, 128, 192])
+def test_tc_eval_adversarial_tables_at_routing_shape(dim):
+    """Every adversarial table of the algorithm model, and products in the fp32 subnormal range, at the shape
+    eval_mf_auto routes to the tensor cores (16 500 items)."""
+    from neurec_b200 import ops
+    from test_tc_algorithm_model import CASES
+    from test_gpu_tc_candidates import make_tables
+    nu, ni, K = 130, 16_500, 10
+    for case in sorted(CASES) + ["subnormal"]:
+        U, V = make_tables(case, nu, ni, dim, seed=dim + len(case))
+        rs = np.random.RandomState(dim)
+        tp, ti = random_csr(rs, nu, ni, rs.randint(0, 40, nu))
+        sp, si = random_csr(rs, nu, ni, rs.randint(1, 12, nu))
+        users = np.arange(nu, dtype=np.int32)
+        want, wranks = oracle.eval_mf(U, V, users, tp, ti, sp, si, ALL, K, thread_num=8, return_ranks=True)
+        got, ranks = ops.eval_mf_tc(dev(U), dev(V), dev(users), dev(tp), dev(ti), dev(sp), dev(si), ALL, K,
+                                    return_ranks=True)
+        assert np.array_equal(ranks.cpu().numpy(), wranks), case
+        assert np.array_equal(got.cpu().numpy(), want), case
