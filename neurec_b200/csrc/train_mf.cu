@@ -165,12 +165,8 @@ struct RowShards {
     float* base[8];
     int32_t rows_per_shard;   // 0: a single local table at base[0]
     int32_t self;             // this rank's shard (rows of other shards live in peer memory)
-    int32_t vec_remote;       // how rows of OTHER ranks are updated: 0 scalar REDs, 1 vector REDs (default), 2 one bulk
-                              // reduce-add of the whole row (cp.reduce.async.bulk from shared memory) -- NRC_PEER_VEC_RED.
+    int32_t vec_remote;       // how rows of OTHER ranks are updated: 0 scalar REDs, otherwise vector REDs -- NRC_PEER_VEC_RED (default 1)
     int32_t force_remote;     // debug (NRC_FORCE_REMOTE_PATH=1): take the remote update path for local item rows too
-    int32_t local_bulk;       // CSR-fed kernel: local rows (user rows, own item rows, the head's delta rows) are updated by ONE
-                              // bulk reduce-add of the staged delta row (cp.reduce.async.bulk .add.f32) instead of 32 vector REDs
-                              // -- NRC_SGD_LOCAL_BULK, default 1
     // Replicated head (n_hot > 0): rows [0, n_hot) -- the loader relabels items by descending train degree, so these
     // are the most popular ones -- are READ from this rank's replica `hot` (L2-resident) and their deltas are
     // accumulated into this rank's `hot_delta`; the caller all-reduces hot_delta between steps and applies it
@@ -307,11 +303,14 @@ static int launch_bpr_sgd(const RowShards& SU, const RowShards& SV, int dim, con
 // The same single-pass step fed straight from the train CSR: positions [first, first + count) of
 // the shuffled epoch (epoch.cuh) are sampled INSIDE the kernel -- no id arrays in HBM, no sampler
 // or shuffle pass in front (data/sampler.py:71-90,189-206 + util/data_iterator.py:59 fused in).
-// A CTA takes 256 consecutive positions at a time:
+// A persistent grid (as many 256-thread CTAs as fit, 3 per SM) splits [first, first + count) evenly;
+// a CTA takes its share 256 consecutive positions at a time:
 //   phase a  one THREAD per triplet: bijection -> (user, positive) -> Philox rejection draw against
 //            the user's sorted row; ~10 dependent loads, 256 chains in flight per CTA;
 //   phase b  one WARP per triplet, two triplets in flight per warp: row gathers (float4 per lane),
-//            shuffle-reduced dots, in-place vector RED.ADD.
+//            shuffle-reduced dots, in-place vector RED.ADD (the hottest head rows: shared memory, below).
+// On one H100 vector REDs were as fast as one bulk reduce-add per row (cp.reduce.async.bulk) and need
+// no staging buffer (profiles/r3_sgd_breakdown_n1.json).
 // User rows are always local (the train CSR is sharded by user owner, SURVEY 8e); item rows may
 // live on any rank (RowShards) and are then read / RED-updated over NVLink by the same kernel.
 // ----------------------------------------------------------------------------------------
@@ -335,112 +334,126 @@ __device__ __forceinline__ void st_vec(float* p, const float (&v)[VEC]) {
     else *p = v[0];
 }
 
-// In-place update of the three rows of one triplet, each by its own mode: 0 scalar REDs, 1 vector REDs, 2 ONE bulk
-// reduce-add of the whole row (cp.reduce.async.bulk ... .add.f32) from the warp's staging rows -- a single transaction
-// per row for the L2 (or over NVLink) instead of 32 x VEC REDs.  The bulk rows of a triplet share one proxy fence,
-// one warp barrier and one bulk group.  p*: lane-offset row pointers (lane 0's is the start of the row).
+// Rows [0, T) of the replicated head are held in shared memory for the whole launch, T = 32 KB of rows (64 at
+// d = 128).  They are the most popular items: at the benchmark's Zipf(1.05) law the top 64 take ~11 % of all row
+// updates of a 2^20-triplet step, row 0 alone ~64 000, and every in-place update of one of them is a same-address
+// atomic serialised in one L2 slice.  Each CTA reads them from its own copy and sums its deltas with shared-memory
+// atomics, so such a row receives one global reduce-add per CTA instead of one per occurrence.
 template <int VEC>
-__device__ __forceinline__ void update_rows3(float* p0, const float (&d0)[VEC], int m0, float* p1, const float (&d1)[VEC], int m1,
-                                             float* p2, const float (&d2)[VEC], int m2, float* stage, int lane) {
-    constexpr int D = 32 * VEC;
-    if (m0 == 2) st_vec<VEC>(stage + lane * VEC, d0); else red_row<VEC>(p0, d0, m0 == 0);
-    if (m1 == 2) st_vec<VEC>(stage + D + lane * VEC, d1); else red_row<VEC>(p1, d1, m1 == 0);
-    if (m2 == 2) st_vec<VEC>(stage + 2 * D + lane * VEC, d2); else red_row<VEC>(p2, d2, m2 == 0);
-    if (m0 == 2 || m1 == 2 || m2 == 2) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) {
-            const uint32_t saddr = (uint32_t)__cvta_generic_to_shared(stage);
-            constexpr uint32_t kBytes = (uint32_t)(D * 4);
-            if (m0 == 2) asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-                                      ::"l"(p0), "r"(saddr), "r"(kBytes) : "memory");
-            if (m1 == 2) asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-                                      ::"l"(p1), "r"(saddr + kBytes), "r"(kBytes) : "memory");
-            if (m2 == 2) asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
-                                      ::"l"(p2), "r"(saddr + 2 * kBytes), "r"(kBytes) : "memory");
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
+constexpr int kSgdTierRows = 8192 / (32 * VEC);
+template <int VEC>
+constexpr size_t kSgdTierBytes = (size_t)2 * kSgdTierRows<VEC> * 32 * VEC * sizeof(float);   // values + deltas
+
+// an item row into registers: from the shared-memory tier (id < nt) or from global / peer memory
+template <int VEC, bool SHARDED>
+__device__ __forceinline__ void load_item(const RowShards& V, int32_t id, int nt, const float* s_val, int lane,
+                                          float (&v)[VEC]) {
+    if (id < nt) {
+        ld_vec<VEC>(s_val + id * (32 * VEC) + lane * VEC, v);
+    } else {
+        bool remote;
+        float* upd;
+        ld_vec<VEC>(V.row<SHARDED>(id, 32 * VEC, remote, upd) + lane * VEC, v);
+    }
+}
+
+// an item row's delta: shared-memory atomics into the tier (element lane*VEC + t of the row at t*32 + lane, so the
+// 32 lanes hit 32 banks), else vector REDs in place (scalar REDs for peer rows when vec_remote == 0)
+template <int VEC, bool SHARDED>
+__device__ __forceinline__ void update_item(const RowShards& V, int32_t id, int nt, float* s_dlt, int lane,
+                                            const float (&d)[VEC]) {
+    if (id < nt) {
+#pragma unroll
+        for (int t = 0; t < VEC; ++t) atomicAdd(s_dlt + id * (32 * VEC) + t * 32 + lane, d[t]);
+    } else {
+        bool remote;
+        float* upd;
+        V.row<SHARDED>(id, 32 * VEC, remote, upd);
+        red_row<VEC>(upd + lane * VEC, d, remote && V.vec_remote == 0);
     }
 }
 
 template <int VEC, bool SHARDED>
-__global__ void __launch_bounds__(256, 4)
+__global__ void __launch_bounds__(256, 3)
 mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const EpochSpec E, int64_t first,
                          int64_t count, float lr, float reg, float* __restrict__ loss) {
-    constexpr int D = 32 * VEC;
-    constexpr int CH = 256;
+    constexpr int D = 32 * VEC, CH = 256, T = kSgdTierRows<VEC>;
+    constexpr int TPW = 2;                     // triplets in flight per warp (3 and 4 measured slower)
     __shared__ int32_t s_u[CH], s_i[CH], s_j[CH];
-    __shared__ __align__(16) float s_stage[8][6][D];      // bulk-reduce staging: 6 rows per warp (2 triplets x 3 rows)
+    extern __shared__ __align__(16) float s_tier[];
+    float* const s_val = s_tier;               // [T][D] pre-step values of head rows [0, nt)
+    float* const s_dlt = s_tier + T * D;       // [T][D] this CTA's summed deltas of those rows
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int rmode = V.vec_remote;
-    const int lmode = V.local_bulk ? 2 : 1;              // update mode of LOCAL rows: 2 bulk reduce-add, 1 vector RED
-    const bool any_bulk = (lmode == 2) || (rmode == 2);
+    const int nt = V.n_hot < T ? V.n_hot : T;
+    for (int e = threadIdx.x; e < nt * D / 4; e += blockDim.x) {
+        reinterpret_cast<float4*>(s_val)[e] = reinterpret_cast<const float4*>(V.hot)[e];
+        reinterpret_cast<float4*>(s_dlt)[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    // an even share of [0, count) per CTA of the persistent grid, sampled 256 positions at a time
+    const int64_t lo = count * blockIdx.x / gridDim.x, hi = count * (blockIdx.x + 1) / gridDim.x;
     float loss_acc = 0.0f;
-    for (int64_t c0 = (int64_t)blockIdx.x * CH; c0 < count; c0 += (int64_t)gridDim.x * CH) {
-        const int n = (count - c0 < CH) ? (int)(count - c0) : CH;
+    for (int64_t c0 = lo; c0 < hi; c0 += CH) {
+        const int n = (hi - c0 < CH) ? (int)(hi - c0) : CH;
         if ((int)threadIdx.x < n) {
             int32_t u, i, j;
             epoch_sample(E, first + c0 + threadIdx.x, 0, u, i, j);
             s_u[threadIdx.x] = u; s_i[threadIdx.x] = i; s_j[threadIdx.x] = j;
         }
         __syncthreads();
-        for (int t0 = warp * 2; t0 < n; t0 += 16) {
-            const bool two = t0 + 1 < n;
-            const int t1 = two ? t0 + 1 : t0;
-            bool ri0, rj0, ri1, rj1;
-            float* pu0 = U_local + (size_t)s_u[t0] * D + lane * VEC;
-            float* pu1 = U_local + (size_t)s_u[t1] * D + lane * VEC;
-            float *wi0, *wj0, *wi1, *wj1;      // where the deltas go (the row itself unless it is replicated)
-            float* qi0 = V.row<SHARDED>(s_i[t0], D, ri0, wi0) + lane * VEC;
-            float* qj0 = V.row<SHARDED>(s_j[t0], D, rj0, wj0) + lane * VEC;
-            float* qi1 = V.row<SHARDED>(s_i[t1], D, ri1, wi1) + lane * VEC;
-            float* qj1 = V.row<SHARDED>(s_j[t1], D, rj1, wj1) + lane * VEC;
-            wi0 += lane * VEC; wj0 += lane * VEC; wi1 += lane * VEC; wj1 += lane * VEC;
-            float a0[VEC], b0[VEC], c0v[VEC], a1[VEC], b1[VEC], c1v[VEC];
-            ld_vec<VEC>(pu0, a0); ld_vec<VEC>(qi0, b0); ld_vec<VEC>(qj0, c0v);
-            ld_vec<VEC>(pu1, a1); ld_vec<VEC>(qi1, b1); ld_vec<VEC>(qj1, c1v);
-            float di0 = 0.f, dj0 = 0.f, sq0 = 0.f, di1 = 0.f, dj1 = 0.f, sq1 = 0.f;
+        // TPW triplets per warp in flight: all 3 * TPW row loads are issued before the first is used
+        for (int t0 = warp * TPW; t0 < n; t0 += 8 * TPW) {
+            float a[TPW][VEC], b[TPW][VEC], c[TPW][VEC];
 #pragma unroll
-            for (int t = 0; t < VEC; ++t) {
-                di0 = fmaf(a0[t], b0[t], di0); dj0 = fmaf(a0[t], c0v[t], dj0);
-                sq0 += a0[t] * a0[t] + b0[t] * b0[t] + c0v[t] * c0v[t];
-                di1 = fmaf(a1[t], b1[t], di1); dj1 = fmaf(a1[t], c1v[t], dj1);
-                sq1 += a1[t] * a1[t] + b1[t] * b1[t] + c1v[t] * c1v[t];
+            for (int k = 0; k < TPW; ++k) {
+                const int t = (t0 + k < n) ? t0 + k : t0;
+                ld_vec<VEC>(U_local + (size_t)s_u[t] * D + lane * VEC, a[k]);
+                load_item<VEC, SHARDED>(V, s_i[t], nt, s_val, lane, b[k]);
+                load_item<VEC, SHARDED>(V, s_j[t], nt, s_val, lane, c[k]);
             }
-            di0 = warp_sum(di0); dj0 = warp_sum(dj0); di1 = warp_sum(di1); dj1 = warp_sum(dj1);
-            const float x0 = di0 - dj0, x1 = di1 - dj1;
-            float l0 = (x0 >= 0.f) ? log1pf(expf(-x0)) : (-x0 + log1pf(expf(x0)));
-            float l1 = (x1 >= 0.f) ? log1pf(expf(-x1)) : (-x1 + log1pf(expf(x1)));
-            if (reg != 0.0f) { l0 += reg * 0.5f * warp_sum(sq0); l1 += reg * 0.5f * warp_sum(sq1); }
-            const float g0 = -1.0f / (1.0f + expf(x0)), g1 = -1.0f / (1.0f + expf(x1));
-            if (any_bulk) {     // the staging rows of the previous pair must have been read by the copy engine; waited for
-                                // HERE, behind this pair's loads and arithmetic, not in front of them
-                if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                __syncwarp();
-            }
-            float du[VEC], dvi[VEC], dvj[VEC];
+            float di[TPW], dj[TPW], sq[TPW];
 #pragma unroll
-            for (int t = 0; t < VEC; ++t) {
-                du[t] = -lr * (g0 * (b0[t] - c0v[t]) + reg * a0[t]);
-                dvi[t] = -lr * (g0 * a0[t] + reg * b0[t]);
-                dvj[t] = -lr * (-g0 * a0[t] + reg * c0v[t]);
-            }
-            update_rows3<VEC>(pu0, du, lmode, wi0, dvi, ri0 ? rmode : lmode, wj0, dvj, rj0 ? rmode : lmode, s_stage[warp][0], lane);
-            loss_acc += l0;
-            if (two) {
+            for (int k = 0; k < TPW; ++k) {
+                di[k] = 0.f; dj[k] = 0.f; sq[k] = 0.f;
 #pragma unroll
                 for (int t = 0; t < VEC; ++t) {
-                    du[t] = -lr * (g1 * (b1[t] - c1v[t]) + reg * a1[t]);
-                    dvi[t] = -lr * (g1 * a1[t] + reg * b1[t]);
-                    dvj[t] = -lr * (-g1 * a1[t] + reg * c1v[t]);
+                    di[k] = fmaf(a[k][t], b[k][t], di[k]); dj[k] = fmaf(a[k][t], c[k][t], dj[k]);
+                    sq[k] += a[k][t] * a[k][t] + b[k][t] * b[k][t] + c[k][t] * c[k][t];
                 }
-                update_rows3<VEC>(pu1, du, lmode, wi1, dvi, ri1 ? rmode : lmode, wj1, dvj, rj1 ? rmode : lmode, s_stage[warp][3], lane);
-                loss_acc += l1;
+                di[k] = warp_sum(di[k]); dj[k] = warp_sum(dj[k]);
+            }
+#pragma unroll
+            for (int k = 0; k < TPW; ++k) {
+                if (t0 + k >= n) break;
+                const int t = t0 + k;
+                const float x = di[k] - dj[k];
+                float l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
+                if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq[k]);
+                loss_acc += l;
+                const float g = -1.0f / (1.0f + expf(x));
+                float du[VEC], dvi[VEC], dvj[VEC];
+#pragma unroll
+                for (int q = 0; q < VEC; ++q) {
+                    du[q] = -lr * (g * (b[k][q] - c[k][q]) + reg * a[k][q]);
+                    dvi[q] = -lr * (g * a[k][q] + reg * b[k][q]);
+                    dvj[q] = -lr * (-g * a[k][q] + reg * c[k][q]);
+                }
+                red_row<VEC>(U_local + (size_t)s_u[t] * D + lane * VEC, du, false);
+                update_item<VEC, SHARDED>(V, s_i[t], nt, s_dlt, lane, dvi);
+                update_item<VEC, SHARDED>(V, s_j[t], nt, s_dlt, lane, dvj);
             }
         }
         __syncthreads();
     }
-    if (any_bulk && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all bulk reduces performed
+    __syncthreads();
+    // the tier's deltas: one vector RED per row slice into hot_delta (rows this CTA never touched add nothing)
+    for (int e = threadIdx.x; e < nt * 32; e += blockDim.x) {
+        const int r = e >> 5, l = e & 31;
+        float d[VEC];
+        bool any = false;
+#pragma unroll
+        for (int t = 0; t < VEC; ++t) { d[t] = s_dlt[r * D + t * 32 + l]; any |= d[t] != 0.0f; }
+        if (any) red_row<VEC>(V.hot_delta + (size_t)r * D + l * VEC, d, false);
+    }
     if (lane == 0 && loss) atomicAdd(loss, loss_acc);
 }
 
@@ -619,14 +632,28 @@ static int sgd_pipe_enabled() {
     return g_sgd_pipe;
 }
 
+template <int VEC, bool SH>
+static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E, int64_t first, int64_t count, float lr,
+                         float reg, float* loss, cudaStream_t st) {
+    constexpr size_t smem = kSgdTierBytes<VEC>;
+    static int64_t grid_cap = 0;     // the persistent grid: as many CTAs as fit on the device at once
+    if (!grid_cap) {
+        NRC_CUDA_CHECK(cudaFuncSetAttribute(mf_bpr_sgd_stream_kernel<VEC, SH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem));
+        int per_sm = 0;
+        NRC_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mf_bpr_sgd_stream_kernel<VEC, SH>, 256, smem));
+        NRC_REQUIRE(per_sm > 0, NRC_E_CUDA, "mf_bpr_sgd_stream_kernel does not fit on an SM");
+        grid_cap = (int64_t)per_sm * sm_count();
+    }
+    int64_t blocks = (count + 255) / 256;
+    if (blocks > grid_cap) blocks = grid_cap;
+    mf_bpr_sgd_stream_kernel<VEC, SH><<<(unsigned)blocks, 256, smem, st>>>(U_local, SV, E, first, count, lr, reg, loss);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
 static int launch_bpr_sgd_stream(float* U_local, const RowShards& SV, int dim, const EpochSpec& E, int64_t first,
                                  int64_t count, float lr, float reg, float* loss, cudaStream_t st) {
-    int64_t blocks = (count + 255) / 256;
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    const unsigned gb = (unsigned)blocks;
-#define NRC_LAUNCH_STREAM(VEC, SH) \
-    mf_bpr_sgd_stream_kernel<VEC, SH><<<gb, 256, 0, st>>>(U_local, SV, E, first, count, lr, reg, loss)
     const bool sharded = SV.rows_per_shard != 0;
     if (sgd_pipe_enabled() && !SV.force_remote && (dim == 128 || dim == 64)) {
         if (dim == 128) return sharded ? launch_pipe<4, true>(U_local, SV, E, first, count, lr, reg, loss, st)
@@ -634,12 +661,12 @@ static int launch_bpr_sgd_stream(float* U_local, const RowShards& SV, int dim, c
         return sharded ? launch_pipe<2, true>(U_local, SV, E, first, count, lr, reg, loss, st)
                        : launch_pipe<2, false>(U_local, SV, E, first, count, lr, reg, loss, st);
     }
-    if (dim == 128) { if (sharded) NRC_LAUNCH_STREAM(4, true); else NRC_LAUNCH_STREAM(4, false); }
-    else if (dim == 64) { if (sharded) NRC_LAUNCH_STREAM(2, true); else NRC_LAUNCH_STREAM(2, false); }
-    else { if (sharded) NRC_LAUNCH_STREAM(1, true); else NRC_LAUNCH_STREAM(1, false); }
-#undef NRC_LAUNCH_STREAM
-    NRC_CUDA_CHECK(cudaGetLastError());
-    return NRC_OK;
+#define NRC_STREAM(VEC) (sharded ? launch_stream<VEC, true>(U_local, SV, E, first, count, lr, reg, loss, st) \
+                                 : launch_stream<VEC, false>(U_local, SV, E, first, count, lr, reg, loss, st))
+    if (dim == 128) return NRC_STREAM(4);
+    if (dim == 64) return NRC_STREAM(2);
+    return NRC_STREAM(1);
+#undef NRC_STREAM
 }
 
 // ----------------------------------------------------------------------------------------
@@ -858,9 +885,6 @@ extern "C" int nrc_mf_bpr_sgd_epoch_hot(float* user_table, float* const* item_sh
         if (force < 0) { const char* e = getenv("NRC_FORCE_REMOTE_PATH"); force = e ? atoi(e) : 0; }
         SV.vec_remote = vec;
         SV.force_remote = force;
-        static int bulk = -1;
-        if (bulk < 0) { const char* e = getenv("NRC_SGD_LOCAL_BULK"); bulk = e ? (atoi(e) != 0) : 1; }
-        SV.local_bulk = bulk;
     }
     return launch_bpr_sgd_stream(user_table, SV, dim, E, first, count, lr, reg, loss, as_stream(stream));
 }
