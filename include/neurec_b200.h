@@ -431,12 +431,6 @@ int nrc_mf_bpr_sgd_epoch_hot(float* user_table, float* const* item_shards, int32
                              float* hot, float* hot_delta, int32_t n_hot, void* stream);
 /* hot[e] += hot_delta[e]; hot_delta[e] = 0 for e < n_floats (a multiple of 4; both 16-byte aligned). */
 int nrc_mf_hot_apply(float* hot, float* hot_delta, int64_t n_floats, void* stream);
-/* Which kernel nrc_mf_bpr_sgd_epoch launches for dim 64 / 128.  0 (default): the register form (a CTA samples 256
- * positions, then two triplets per warp in flight: LDG.128 row gathers, shuffle dots, vector RED.ADD).  1: the
- * pipelined form -- sampler warps feed an id queue, consumer warps issue bulk copies (cp.async.bulk) of the three
- * rows into a 128-slot shared-memory ring and return the deltas as vector REDs.  Same arithmetic per triplet.
- * Returns the previous setting.  (NRC_SGD_PIPE=0/1 sets the initial value.) */
-int nrc_mf_sgd_set_pipelined(int32_t on);
 
 
 /* The explicitly-named LAZY-Adam variant of nrc_mf_bpr_sgd_epoch (SURVEY.md 8d, BASELINE configs[4]:

@@ -16,15 +16,15 @@
 //   phase 2  TensorFlow-1.12 optimizer over BOTH tables (float4 per thread; Adam is dense, TF's
 //            _apply_sparse_shared), accumulators zeroed,
 //   grid barrier.
-// Two barriers per step are the minimum TF's semantics allow: every gradient read sees the
-// pre-step tables, and Adam moves every row every step.  The tables (0.7 MB for ml-100k) stay in
+// Two barriers per step keep TF's semantics with each phase a plain pass over its data: every
+// gradient read sees the pre-step tables, and Adam moves every row every step.  The tables (0.7 MB for ml-100k) stay in
 // L2; a step costs two barrier round trips plus ~1 us of latency-bound work instead of two
 // kernel launches and their gaps.
 #include "epoch.cuh"
+#include "mf.cuh"
 #include "optim.cuh"
 
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 namespace nrc {
 
@@ -105,147 +105,8 @@ struct MfEpochParams {
     int64_t first_step, num_steps, steps_total;
     int32_t num_users, num_items, D, batch_size;
     int32_t loss_kind, opt_kind, first_stamp, build;
-    int32_t bar_mode;           // grid_barrier flavour (NRC_BAR_MODE)
-    int32_t dbg;                // NRC_EPOCH_DBG experiment bits (0 in normal use): 1 skip the gradient phase, 2 skip the optimizer phase
     float reg, h0, h1, h2, h3;
 };
-
-__device__ __forceinline__ float neg_log_sigmoid_e(float x) {
-    return (x >= 0.0f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-}
-
-// loss value and dl/dx of one sample; x = score difference (pairwise) or score (pointwise)
-template <bool PAIRWISE>
-__device__ __forceinline__ void sample_loss_grad(int kind, float x, float z, float inv_b, float& l, float& g) {
-    if constexpr (PAIRWISE) {
-        if (kind == NRC_LOSS_BPR) {            // learner.py:21-22
-            l = neg_log_sigmoid_e(x);
-            g = -1.0f / (1.0f + expf(x));
-        } else if (kind == NRC_LOSS_HINGE) {   // learner.py:23-24 [sic]
-            const float t = x + 1.0f;
-            l = fmaxf(t, 0.0f);
-            g = (t > 0.0f) ? 1.0f : 0.0f;
-        } else {                               // learner.py:25-26
-            const float t = 1.0f - x;
-            l = t * t;
-            g = -2.0f * t;
-        }
-    } else {
-        if (kind == NRC_LOSS_CROSS_ENTROPY) {  // learner.py:33-34: mean over the batch
-            const float e = expf(-fabsf(x));
-            l = (fmaxf(x, 0.0f) - x * z + log1pf(e)) * inv_b;
-            const float s = (x >= 0.0f) ? 1.0f / (1.0f + e) : e / (1.0f + e);
-            g = (s - z) * inv_b;
-        } else {                               // learner.py:37-38
-            const float t = z - x;
-            l = t * t;
-            g = -2.0f * t;
-        }
-    }
-}
-
-template <int VEC>
-__device__ __forceinline__ void ld_row(const float* p, float (&v)[VEC]) {
-    if constexpr (VEC == 4) {
-        const float4 x = __ldcg(reinterpret_cast<const float4*>(p));
-        v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
-    } else if constexpr (VEC == 2) {
-        const float2 x = __ldcg(reinterpret_cast<const float2*>(p));
-        v[0] = x.x; v[1] = x.y;
-    } else {
-        v[0] = __ldcg(p);
-    }
-}
-
-template <int VEC>
-__device__ __forceinline__ void red_vec(float* p, const float (&d)[VEC]) {
-    if constexpr (VEC == 4) atomicAdd(reinterpret_cast<float4*>(p), make_float4(d[0], d[1], d[2], d[3]));
-    else if constexpr (VEC == 2) atomicAdd(reinterpret_cast<float2*>(p), make_float2(d[0], d[1]));
-    else atomicAdd(p, d[0]);
-}
-
-// Gradient of one triplet / sample by one warp.  VEC > 0: dim == 32 * VEC, the lane keeps its slice
-// of the rows in registers; VEC == 0: any dim, strided loop.
-template <bool PAIRWISE, int VEC>
-__device__ __forceinline__ float mf_sample_grad(const MfEpochParams& P, int lane, int32_t u, int32_t i, int32_t t,
-                                                float inv_b, int32_t stamp) {
-    const int D = P.D;
-    const float reg = P.reg;
-    const float* pu = P.U + (size_t)u * D;
-    const float* qi = P.V + (size_t)i * D;
-    const float* qj = PAIRWISE ? P.V + (size_t)t * D : nullptr;
-    float* gu = P.gU + (size_t)u * D;
-    float* gi = P.gV + (size_t)i * D;
-    float* gj = PAIRWISE ? P.gV + (size_t)t * D : nullptr;
-    const float z = PAIRWISE ? 0.0f : __int_as_float(t);
-    float l, g;
-    if constexpr (VEC > 0) {
-        const int k0 = lane * VEC;
-        float a[VEC], bi[VEC], bj[VEC];
-        ld_row<VEC>(pu + k0, a);
-        ld_row<VEC>(qi + k0, bi);
-        if constexpr (PAIRWISE) ld_row<VEC>(qj + k0, bj);
-        float di = 0.0f, dj = 0.0f, sq = 0.0f;
-#pragma unroll
-        for (int c = 0; c < VEC; ++c) {
-            di = fmaf(a[c], bi[c], di);
-            if constexpr (PAIRWISE) { dj = fmaf(a[c], bj[c], dj); sq += a[c] * a[c] + bi[c] * bi[c] + bj[c] * bj[c]; }
-            else sq += a[c] * a[c] + bi[c] * bi[c];
-        }
-        di = warp_sum(di);
-        if constexpr (PAIRWISE) dj = warp_sum(dj);
-        sample_loss_grad<PAIRWISE>(P.loss_kind, PAIRWISE ? di - dj : di, z, inv_b, l, g);
-        if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);
-        float du[VEC], dvi[VEC], dvj[VEC];
-#pragma unroll
-        for (int c = 0; c < VEC; ++c) {
-            if constexpr (PAIRWISE) {
-                du[c] = g * (bi[c] - bj[c]) + reg * a[c];
-                dvi[c] = g * a[c] + reg * bi[c];
-                dvj[c] = -g * a[c] + reg * bj[c];
-            } else {
-                du[c] = g * bi[c] + reg * a[c];
-                dvi[c] = g * a[c] + reg * bi[c];
-            }
-        }
-        red_vec<VEC>(gu + k0, du);
-        red_vec<VEC>(gi + k0, dvi);
-        if constexpr (PAIRWISE) red_vec<VEC>(gj + k0, dvj);
-    } else {
-        float di = 0.0f, dj = 0.0f, sq = 0.0f;
-        for (int k = lane; k < D; k += kWarp) {
-            const float a = __ldcg(pu + k), bi = __ldcg(qi + k);
-            di = fmaf(a, bi, di);
-            if constexpr (PAIRWISE) {
-                const float bj = __ldcg(qj + k);
-                dj = fmaf(a, bj, dj);
-                sq += a * a + bi * bi + bj * bj;
-            } else sq += a * a + bi * bi;
-        }
-        di = warp_sum(di);
-        if constexpr (PAIRWISE) dj = warp_sum(dj);
-        sample_loss_grad<PAIRWISE>(P.loss_kind, PAIRWISE ? di - dj : di, z, inv_b, l, g);
-        if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);
-        for (int k = lane; k < D; k += kWarp) {
-            const float a = __ldcg(pu + k), bi = __ldcg(qi + k);
-            if constexpr (PAIRWISE) {
-                const float bj = __ldcg(qj + k);
-                atomicAdd(gu + k, g * (bi - bj) + reg * a);
-                atomicAdd(gi + k, g * a + reg * bi);
-                atomicAdd(gj + k, -g * a + reg * bj);
-            } else {
-                atomicAdd(gu + k, g * bi + reg * a);
-                atomicAdd(gi + k, g * a + reg * bi);
-            }
-        }
-    }
-    if (lane == 0) {
-        P.tU[u] = stamp;
-        P.tV[i] = stamp;
-        if constexpr (PAIRWISE) P.tV[t] = stamp;
-    }
-    return l;
-}
 
 template <bool PAIRWISE, int VEC>
 __global__ void __launch_bounds__(512, 1) mf_epoch_kernel(const MfEpochParams P) {
@@ -263,7 +124,7 @@ __global__ void __launch_bounds__(512, 1) mf_epoch_kernel(const MfEpochParams P)
             P.ws_u[p] = u; P.ws_i[p] = it; P.ws_t[p] = th;
         }
         for (int64_t s = tid; s < P.steps_total; s += nthr) P.step_loss[s] = 0.0f;
-        grid_barrier(P.barrier, target, P.bar_mode);
+        grid_barrier(P.barrier, target);
     }
 
     // TF keeps beta1^t / beta2^t as fp32 variables multiplied once per step (adam.py::_finish)
@@ -282,12 +143,13 @@ __global__ void __launch_bounds__(512, 1) mf_epoch_kernel(const MfEpochParams P)
         // ---- phase 1: gradients of the batch
         const float inv_b = 1.0f / (float)cnt;
         float loss_acc = 0.0f;
-        for (int64_t b = warp_g; b < cnt && !(P.dbg & 1); b += warps) {
+        for (int64_t b = warp_g; b < cnt; b += warps) {
             const int32_t u = __ldcg(P.ws_u + off + b), i = __ldcg(P.ws_i + off + b), t = __ldcg(P.ws_t + off + b);
-            loss_acc += mf_sample_grad<PAIRWISE, VEC>(P, lane, u, i, t, inv_b, stamp);
+            loss_acc += mf_sample_grad<PAIRWISE, VEC, true>(P.U, P.V, P.gU, P.gV, P.tU, P.tV, D, P.reg, P.loss_kind, lane,
+                                                            u, i, t, inv_b, stamp);
         }
         if (lane == 0 && warp_g < cnt) atomicAdd(P.step_loss + s, loss_acc);
-        grid_barrier(P.barrier, target, P.bar_mode);
+        grid_barrier(P.barrier, target);
         // ---- phase 2: optimizer over both tables
         float h0 = P.h0;
         if (adam) {   // lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t), fp32 (adam.py::_prepare)
@@ -295,8 +157,7 @@ __global__ void __launch_bounds__(512, 1) mf_epoch_kernel(const MfEpochParams P)
             p1 = __fmul_rn(p1, P.h1);
             p2 = __fmul_rn(p2, P.h2);
         }
-        if (P.dbg & 2) {
-        } else if ((D & 3) == 0) {
+        if ((D & 3) == 0) {
             for (int64_t e = tid * 4; e < eAll; e += nthr * 4) {
                 const bool isU = e < eU;
                 const int64_t i = isU ? e : e - eU;
@@ -337,215 +198,9 @@ __global__ void __launch_bounds__(512, 1) mf_epoch_kernel(const MfEpochParams P)
                 *grd = 0.0f;
             }
         }
-        grid_barrier(P.barrier, target, P.bar_mode);
+        grid_barrier(P.barrier, target);
     }
     if (adam && tid == 0) { P.adam_pows[0] = p1; P.adam_pows[1] = p2; }
-}
-
-// ----------------------------------------------------------------------------------------
-// ONE grid barrier per step ("pull-based optimizer").  The two-barrier kernel above waits between
-// the optimizer pass of step t-1 and the gradient pass of step t because the gradient pass reads the
-// updated rows.  But the update of a row is a function of that row alone -- (var, slots, gradient of
-// step t-1) -> var' -- so a warp that needs rows u, i, j for step t can apply the pending update to
-// just those three rows in registers, with the very same opt_update() the dense pass runs, instead of
-// waiting for the dense pass to write them back.  With the state double-buffered (the dense pass of
-// step t-1 reads set A and writes set B while the pulling warps read set A) and the gradient
-// accumulators triple-buffered (step t accumulates into G[t%3] while G[(t-1)%3] is being read and
-// G[(t+1)%3] is being zeroed), the optimizer pass of step t-1 and the gradient pass of step t run in
-// the SAME phase: per step  { dense optimizer(t-1)  ||  gradients(t) with pulled rows } -> barrier.
-// Same arithmetic, element for element, as the two-barrier kernel (tests compare both).
-// ----------------------------------------------------------------------------------------
-struct MfStateSet {
-    float* U; float* V; float* s0U; float* s1U; float* s0V; float* s1V;
-};
-
-struct MfEpoch1Params {
-    MfEpochParams B;              // everything of the two-barrier kernel (its U/V/slots = state set 0, gU/gV = G[0], tU/tV = stamps[0])
-    MfStateSet set1;              // scratch state set 1
-    float* gU12[2]; float* gV12[2];   // scratch gradient accumulators G[1], G[2] (zero on entry)
-    int32_t* tU1; int32_t* tV1;   // scratch stamp arrays (set 1)
-};
-
-// one lane's slice of a row with the pending optimizer step applied (or as stored when none is pending)
-template <int VEC>
-__device__ __forceinline__ void pull_row(const float* var, const float* g, const float* s0, const float* s1, bool pending,
-                                         bool touched, int kind, float h0, float h1, float h2, float h3, float (&out)[VEC]) {
-    ld_row<VEC>(var, out);
-    if (!pending) return;
-    float gv[VEC], a[VEC], c[VEC];
-    ld_row<VEC>(g, gv);
-    const bool has0 = kind != NRC_OPT_GD, has1 = kind == NRC_OPT_ADAM || kind == NRC_OPT_RMSPROP;
-    if (has0) ld_row<VEC>(s0, a);
-    if (has1) ld_row<VEC>(s1, c);
-#pragma unroll
-    for (int t = 0; t < VEC; ++t) {
-        float aa = has0 ? a[t] : 0.0f, cc = has1 ? c[t] : 0.0f;
-        opt_update(kind, 0, touched, h0, h1, h2, h3, out[t], gv[t], aa, cc);
-    }
-}
-
-template <bool PAIRWISE, int VEC>
-__global__ void __launch_bounds__(512, 1) mf_epoch1_kernel(const MfEpoch1Params Q) {
-    const MfEpochParams& P = Q.B;
-    const int lane = threadIdx.x & 31;
-    const int64_t warp_g = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int64_t warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t nthr = (int64_t)gridDim.x * blockDim.x;
-    unsigned int target = 0;
-    constexpr int D = 32 * VEC;
-
-    if (P.build) {
-        for (int64_t p = tid; p < P.n_used; p += nthr) {
-            int32_t u, it, th;
-            epoch_sample(P.E, p, 0, u, it, th);
-            P.ws_u[p] = u; P.ws_i[p] = it; P.ws_t[p] = th;
-        }
-        for (int64_t s = tid; s < P.steps_total; s += nthr) P.step_loss[s] = 0.0f;
-        grid_barrier(P.barrier, target, P.bar_mode);
-    }
-    const bool adam = P.opt_kind == NRC_OPT_ADAM;
-    const bool stamped = !(adam || P.opt_kind == NRC_OPT_GD);
-    float p1 = 0.0f, p2 = 0.0f;
-    if (adam) { p1 = __ldcg(P.adam_pows); p2 = __ldcg(P.adam_pows + 1); }
-    const bool has0 = P.opt_kind != NRC_OPT_GD;
-    const bool has1 = adam || P.opt_kind == NRC_OPT_RMSPROP;
-    const int64_t eU = (int64_t)P.num_users * D, eAll = eU + (int64_t)P.num_items * D;
-    // rotating roles (kept in registers, swapped after every barrier):
-    //   cur / alt      state set holding the values BEFORE the pending update / the set the dense pass writes
-    //   g_pend / g_cur / g_zero   gradient of the pending step / of this step / being zeroed for the next
-    //   tp / tc        stamp arrays of the pending step / of this step
-    MfStateSet cur = {P.U, P.V, P.s0U, P.s1U, P.s0V, P.s1V}, alt = Q.set1;
-    const MfStateSet home = cur;
-    float *gU_pend = Q.gU12[1], *gV_pend = Q.gV12[1], *gU_cur = P.gU, *gV_cur = P.gV, *gU_zero = Q.gU12[0], *gV_zero = Q.gV12[0];
-    int32_t *tUp = Q.tU1, *tVp = Q.tV1, *tUc = P.tU, *tVc = P.tV;
-    const int T = (int)P.num_steps;
-
-    for (int t = 0; t <= T; ++t) {
-        // hyper-parameters of the PENDING step t-1
-        float h0 = P.h0;
-        if (t >= 1 && adam) {
-            h0 = __fdiv_rn(__fmul_rn(P.h0, __fsqrt_rn(__fsub_rn(1.0f, p2))), __fsub_rn(1.0f, p1));
-            p1 = __fmul_rn(p1, P.h1);
-            p2 = __fmul_rn(p2, P.h2);
-        }
-        const bool pending = t >= 1, last = t == T;
-        const MfStateSet dst = last ? home : alt;               // the last pass lands in the caller's buffers (in place if it must)
-        const int32_t stamp_prev = P.first_stamp + t - 1, stamp_cur = P.first_stamp + t;
-        // ---- dense optimizer pass of step t-1: cur -> dst; zero the accumulator of step t+1 (all of them in the last pass)
-        // Roles.  When the batch needs at most half of the grid's warps, every `gstride`-th warp takes one
-        // triplet of step t (so the gradient warps are spread over all SMs) and ALL OTHER warps run the dense
-        // pass of step t-1 at the same time; otherwise every warp does the dense pass and then its triplets.
-        int64_t cnt_t = 0;
-        if (!last) {
-            const int64_t off_t = (P.first_step + t) * P.batch_size;
-            cnt_t = (P.n_used - off_t < P.batch_size) ? (P.n_used - off_t) : P.batch_size;
-        }
-        const bool split = pending && !last && cnt_t * 2 <= warps;
-        const int64_t gstride = split ? warps / cnt_t : 1;
-        const bool grad_warp = split ? (warp_g % gstride == 0 && warp_g / gstride < cnt_t) : true;
-        int64_t d_tid = tid, d_nthr = nthr;                    // dense-pass worker id / count
-        if (split) {
-            const int64_t before = (warp_g / gstride + 1 < cnt_t) ? (warp_g / gstride + 1) : cnt_t;   // gradient warps with index <= mine
-            d_tid = (warp_g - before) * 32 + lane;
-            d_nthr = (warps - cnt_t) * 32;
-        }
-        if (pending && !(split && grad_warp)) {
-            for (int64_t e = d_tid * 4; e < eAll; e += d_nthr * 4) {
-                const bool isU = e < eU;
-                const int64_t i = isU ? e : e - eU;
-                const float4 g = __ldcg(reinterpret_cast<const float4*>((isU ? gU_pend : gV_pend) + i));
-                float4 v = __ldcg(reinterpret_cast<const float4*>((isU ? cur.U : cur.V) + i));
-                float4 a = has0 ? __ldcg(reinterpret_cast<const float4*>((isU ? cur.s0U : cur.s0V) + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                float4 c = has1 ? __ldcg(reinterpret_cast<const float4*>((isU ? cur.s1U : cur.s1V) + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                const bool touched = stamped ? (__ldcg((isU ? tUp : tVp) + i / D) == stamp_prev) : true;
-                opt_update(P.opt_kind, 0, touched, h0, P.h1, P.h2, P.h3, v.x, g.x, a.x, c.x);
-                opt_update(P.opt_kind, 0, touched, h0, P.h1, P.h2, P.h3, v.y, g.y, a.y, c.y);
-                opt_update(P.opt_kind, 0, touched, h0, P.h1, P.h2, P.h3, v.z, g.z, a.z, c.z);
-                opt_update(P.opt_kind, 0, touched, h0, P.h1, P.h2, P.h3, v.w, g.w, a.w, c.w);
-                *reinterpret_cast<float4*>((isU ? dst.U : dst.V) + i) = v;
-                if (has0) *reinterpret_cast<float4*>((isU ? dst.s0U : dst.s0V) + i) = a;
-                if (has1) *reinterpret_cast<float4*>((isU ? dst.s1U : dst.s1V) + i) = c;
-                const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                *reinterpret_cast<float4*>((isU ? gU_zero : gV_zero) + i) = z4;
-                if (last) *reinterpret_cast<float4*>((isU ? gU_pend : gV_pend) + i) = z4;
-            }
-        }
-        if (last) break;
-        // ---- gradients of step t on rows with the pending update pulled in
-        const int64_t s = P.first_step + t;
-        const int64_t off = s * P.batch_size;
-        const int64_t cnt = cnt_t;
-        const float inv_b = 1.0f / (float)cnt;
-        float loss_acc = 0.0f;
-        const int64_t b0 = split ? (grad_warp ? warp_g / gstride : cnt) : warp_g;
-        const int64_t bstep = split ? cnt : warps;
-        for (int64_t b = b0; b < cnt; b += bstep) {
-            const int32_t u = __ldcg(P.ws_u + off + b), i = __ldcg(P.ws_i + off + b), th = __ldcg(P.ws_t + off + b);
-            const size_t ou = (size_t)u * D + lane * VEC, oi = (size_t)i * D + lane * VEC;
-            const size_t oj = PAIRWISE ? (size_t)th * D + lane * VEC : 0;
-            float a[VEC], bi[VEC], bj[VEC];
-            const bool tu = (stamped && pending) ? (__ldcg(tUp + u) == stamp_prev) : true;
-            const bool ti = (stamped && pending) ? (__ldcg(tVp + i) == stamp_prev) : true;
-            pull_row<VEC>(cur.U + ou, gU_pend + ou, cur.s0U + ou, cur.s1U + ou, pending, tu, P.opt_kind, h0, P.h1, P.h2, P.h3, a);
-            pull_row<VEC>(cur.V + oi, gV_pend + oi, cur.s0V + oi, cur.s1V + oi, pending, ti, P.opt_kind, h0, P.h1, P.h2, P.h3, bi);
-            if constexpr (PAIRWISE) {
-                const bool tj = (stamped && pending) ? (__ldcg(tVp + th) == stamp_prev) : true;
-                pull_row<VEC>(cur.V + oj, gV_pend + oj, cur.s0V + oj, cur.s1V + oj, pending, tj, P.opt_kind, h0, P.h1, P.h2, P.h3, bj);
-            }
-            float di = 0.0f, dj = 0.0f, sq = 0.0f;
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) {
-                di = fmaf(a[c], bi[c], di);
-                if constexpr (PAIRWISE) { dj = fmaf(a[c], bj[c], dj); sq += a[c] * a[c] + bi[c] * bi[c] + bj[c] * bj[c]; }
-                else sq += a[c] * a[c] + bi[c] * bi[c];
-            }
-            di = warp_sum(di);
-            if constexpr (PAIRWISE) dj = warp_sum(dj);
-            float l, g;
-            sample_loss_grad<PAIRWISE>(P.loss_kind, PAIRWISE ? di - dj : di, PAIRWISE ? 0.0f : __int_as_float(th), inv_b, l, g);
-            if (P.reg != 0.0f) l += P.reg * 0.5f * warp_sum(sq);
-            loss_acc += l;
-            float du[VEC], dvi[VEC], dvj[VEC];
-#pragma unroll
-            for (int c = 0; c < VEC; ++c) {
-                if constexpr (PAIRWISE) {
-                    du[c] = g * (bi[c] - bj[c]) + P.reg * a[c];
-                    dvi[c] = g * a[c] + P.reg * bi[c];
-                    dvj[c] = -g * a[c] + P.reg * bj[c];
-                } else {
-                    du[c] = g * bi[c] + P.reg * a[c];
-                    dvi[c] = g * a[c] + P.reg * bi[c];
-                }
-            }
-            red_vec<VEC>(gU_cur + ou, du);
-            red_vec<VEC>(gV_cur + oi, dvi);
-            if constexpr (PAIRWISE) red_vec<VEC>(gV_cur + oj, dvj);
-            if (lane == 0) {
-                tUc[u] = stamp_cur; tVc[i] = stamp_cur;
-                if constexpr (PAIRWISE) tVc[th] = stamp_cur;
-            }
-        }
-        if (lane == 0 && b0 < cnt) atomicAdd(P.step_loss + s, loss_acc);
-        grid_barrier(P.barrier, target, P.bar_mode);
-        // rotate the roles
-        if (pending) { const MfStateSet x = cur; cur = alt; alt = x; }
-        { float* x = gU_pend; gU_pend = gU_cur; gU_cur = gU_zero; gU_zero = x; }
-        { float* x = gV_pend; gV_pend = gV_cur; gV_cur = gV_zero; gV_zero = x; }
-        { int32_t* x = tUp; tUp = tUc; tUc = x; }
-        { int32_t* x = tVp; tVp = tVc; tVc = x; }
-    }
-    if (adam && tid == 0) { P.adam_pows[0] = p1; P.adam_pows[1] = p2; }
-}
-
-// scratch of the one-barrier kernel: state set 1, two gradient accumulators, one stamp set
-static float* g_e1_buf = nullptr;
-static size_t g_e1_floats = 0;
-
-int epoch_bar_mode() {
-    static int mode = -1;
-    if (mode < 0) { const char* e = getenv("NRC_BAR_MODE"); mode = e ? atoi(e) : 0; }   // 0: the default grid-barrier flavour
-    return mode;
 }
 
 // per-device barrier word of the persistent kernels
@@ -646,12 +301,6 @@ extern "C" int nrc_mf_epoch_fused(float* user_table, float* item_table, int32_t 
     P.num_users = num_users; P.num_items = num_items; P.D = dim; P.batch_size = batch_size;
     P.loss_kind = loss_kind; P.opt_kind = opt_kind; P.first_stamp = first_stamp;
     P.build = first_step == 0 ? 1 : 0;
-    {
-        static int dbg = -1;
-        if (dbg < 0) { const char* e = getenv("NRC_EPOCH_DBG"); dbg = e ? atoi(e) : 0; }
-        P.dbg = dbg;
-    }
-    P.bar_mode = epoch_bar_mode();
     P.reg = reg;
     P.h0 = hyper_host ? hyper_host[0] : 0.0f; P.h1 = hyper_host ? hyper_host[1] : 0.0f;
     P.h2 = hyper_host ? hyper_host[2] : 0.0f; P.h3 = hyper_host ? hyper_host[3] : 0.0f;
@@ -659,48 +308,6 @@ extern "C" int nrc_mf_epoch_fused(float* user_table, float* item_table, int32_t 
     if (rc) return rc;
     cudaStream_t st = as_stream(stream);
     NRC_CUDA_CHECK(cudaMemsetAsync(P.barrier, 0, sizeof(unsigned int), st));
-
-    // Default: the two-barrier kernel.  The one-barrier (pull-based) kernel is correct and tested
-    // (NRC_EPOCH_TWO_BARRIER=0): the pull (12 row loads + the optimizer math on three rows per triplet, in the
-    // critical path of every gradient warp) sits where the second grid barrier was.
-    static int two_barrier = -1;
-    if (two_barrier < 0) { const char* e = getenv("NRC_EPOCH_TWO_BARRIER"); two_barrier = e ? atoi(e) : 1; }
-    if (!two_barrier && !P.dbg && (dim == 32 || dim == 64 || dim == 128)) {
-        // one barrier per step: scratch = state set 1 (var + slots of both tables), G[1], G[2], stamps set 1
-        const size_t eAll = (size_t)(num_users + num_items) * dim;
-        const size_t need = eAll * 5 + (size_t)num_users + num_items + 64;
-        if (need > g_e1_floats) {
-            if (g_e1_buf) NRC_CUDA_CHECK(cudaFree(g_e1_buf));
-            g_e1_buf = nullptr; g_e1_floats = 0;
-            NRC_CUDA_CHECK(cudaMalloc(&g_e1_buf, need * sizeof(float)));
-            g_e1_floats = need;
-        }
-        MfEpoch1Params Q;
-        Q.B = P;
-        float* w = g_e1_buf;
-        const size_t nU = (size_t)num_users * dim, nV = (size_t)num_items * dim;
-        Q.set1.U = w; w += nU; Q.set1.V = w; w += nV;
-        Q.set1.s0U = w; w += nU; Q.set1.s0V = w; w += nV;
-        Q.set1.s1U = w; w += nU; Q.set1.s1V = w; w += nV;
-        float* gz = w;
-        Q.gU12[0] = w; w += nU; Q.gV12[0] = w; w += nV;
-        Q.gU12[1] = w; w += nU; Q.gV12[1] = w; w += nV;
-        Q.tU1 = reinterpret_cast<int32_t*>(w); Q.tV1 = Q.tU1 + num_users;
-        NRC_CUDA_CHECK(cudaMemsetAsync(gz, 0, (2 * eAll + num_users + num_items) * sizeof(float), st));
-        const void* fn1;
-#define NRC_PICK1(PW) \
-        fn1 = dim == 128 ? (const void*)mf_epoch1_kernel<PW, 4> : dim == 64 ? (const void*)mf_epoch1_kernel<PW, 2> \
-            : (const void*)mf_epoch1_kernel<PW, 1>
-        if (pairwise) { NRC_PICK1(true); } else { NRC_PICK1(false); }
-#undef NRC_PICK1
-        int per_sm1 = 0;
-        NRC_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm1, fn1, 512, 0));
-        NRC_REQUIRE(per_sm1 >= 1, NRC_E_CUDA, "the persistent epoch kernel does not fit an SM");
-        void* args1[] = {&Q};
-        NRC_CUDA_CHECK(cudaLaunchCooperativeKernel(fn1, dim3(sm_count()), dim3(512), args1, 0, st));
-        return NRC_OK;
-    }
-
     const void* fn;
 #define NRC_PICK(PW) \
     fn = dim == 128 ? (const void*)mf_epoch_kernel<PW, 4> : dim == 64 ? (const void*)mf_epoch_kernel<PW, 2> \

@@ -114,38 +114,19 @@ int epoch_spec_init(EpochSpec& E, const int64_t* tptr, const int32_t* tidx, cons
 
 // Grid-wide barrier of a cooperative launch (all CTAs co-resident).  `counter` counts arrivals
 // monotonically from 0 at kernel start; the k-th barrier completes when it reaches k * gridDim.x.
-// bar.sync orders every thread's earlier writes / REDs before thread 0's release fence
-// (fence cumulativity), thread 0's acquire fence orders them before every later read of the CTA.
-// mode (NRC_BAR_MODE, measurement knob): 0 release-RED + acquire-load polling; 1 fence + relaxed atomic +
-// volatile polling + fence (cooperative-groups style); 2 release-RED + relaxed polling + one acquire fence.
-__device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int& target, int mode = 0) {
+// bar.sync orders every thread's earlier writes / REDs before thread 0's release-arrive (fence
+// cumulativity); thread 0's acquire-load polling orders them before every later read of the CTA.
+__device__ __forceinline__ void grid_barrier(unsigned int* counter, unsigned int& target) {
     __syncthreads();
     if (threadIdx.x == 0) {
         target += gridDim.x;
         unsigned int seen;
-        if (mode == 1) {
-            __threadfence();
-            atomicAdd(counter, 1u);
-            do { seen = *reinterpret_cast<volatile unsigned int*>(counter); } while (seen < target);
-            __threadfence();
-        } else {
-            // release-arrive: orders everything the CTA wrote before its bar.sync (fence cumulativity)
-            asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-            if (mode == 0) {
-                do {
-                    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-                } while (seen < target);
-            } else {
-                do {
-                    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-                } while (seen < target);
-                asm volatile("fence.acq_rel.gpu;" ::: "memory");
-            }
-        }
+        asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
+        do {
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
+        } while (seen < target);
     }
     __syncthreads();
 }
-
-int epoch_bar_mode();   // epoch.cu: NRC_BAR_MODE, default 0
 
 }  // namespace nrc

@@ -15,6 +15,7 @@
 // s_uk = 1 + #{trusted f : social item in train(f)} (SBPR.py:141-145).
 #include "common.cuh"
 #include "epoch.cuh"
+#include "learner.cuh"
 #include "optim.cuh"
 #include "philox.cuh"
 
@@ -104,16 +105,6 @@ sbpr_epoch_build_kernel(const SbprSpec S, int64_t first, int64_t count, int32_t*
     }
 }
 
-__device__ __forceinline__ float neg_log_sigmoid_x(float x) {
-    return (x >= 0.0f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-}
-
-__device__ __forceinline__ void pairwise_loss_grad_x(int kind, float x, float& l, float& g) {
-    if (kind == NRC_LOSS_BPR) { l = neg_log_sigmoid_x(x); g = -1.0f / (1.0f + expf(x)); }         // learner.py:21-22
-    else if (kind == NRC_LOSS_HINGE) { const float t = x + 1.0f; l = fmaxf(t, 0.0f); g = (t > 0.0f) ? 1.0f : 0.0f; }   // :23-24 [sic]
-    else { const float t = 1.0f - x; l = t * t; g = -2.0f * t; }                                   // :25-26
-}
-
 // One warp per (user, positive, social, negative, s_uk) sample.  SBPR.py:66-92:
 //   x_* = <p, q_*> + b_*;  r1 = (x_i - x_k) / s;  r2 = x_k - x_j
 //   loss = l(r1) + l(r2) + reg * l2_loss(p, q_k, q_i, q_j, b_i, b_k, b_j)
@@ -145,8 +136,8 @@ sbpr_grad_kernel(const float* __restrict__ U, const float* __restrict__ V, const
         const float bi = B[i], bk = B[k], bj = B[j];
         const float xi = di + bi, xk = dk + bk, xj = dj + bj;
         float l1, g1, l2, g2;
-        pairwise_loss_grad_x(loss_kind, (xi - xk) / s, l1, g1);
-        pairwise_loss_grad_x(loss_kind, xk - xj, l2, g2);
+        pairwise_loss_grad(loss_kind, (xi - xk) / s, l1, g1);
+        pairwise_loss_grad(loss_kind, xk - xj, l2, g2);
         float l = l1 + l2;
         if (reg != 0.0f) l += reg * 0.5f * (warp_sum(sq) + bi * bi + bk * bk + bj * bj);
         loss_acc += l;

@@ -22,6 +22,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "learner.cuh"
 #include "optim.cuh"
 
 namespace nrc {
@@ -349,9 +350,9 @@ lightgcn_grad_kernel(const float* __restrict__ E, const float* __restrict__ E0, 
         }
         di = warp_sum(di); dj = warp_sum(dj); sq = warp_sum(sq);
         const float x = di - dj;
-        mf_acc += (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
+        mf_acc += neg_log_sigmoid(x);
         emb_acc += reg * 0.5f * sq;
-        const float g = -1.0f / (1.0f + expf(x)) * scale;
+        const float g = neg_log_sigmoid_grad(x) * scale;
         for (int k = lane; k < D; k += kWarp) {
             const float a = E[ru + k], bi = E[ri + k], bj = E[rj + k];
             atomicAdd(G + ru + k, g * (bi - bj));

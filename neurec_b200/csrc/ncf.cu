@@ -26,6 +26,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "learner.cuh"
 #include "ncf.cuh"
 #include "optim.cuh"
 
@@ -123,28 +124,10 @@ ncf_sample_kernel(const NcfDev S, const NcfPtrs P, const int32_t* __restrict__ u
     }
 
     float l, g;
-    if (pairwise) {
-        const float x = yhat[0] - yhat[1];  // NeuMF.py:92 result = output - output_neg
-        if (loss_kind == NRC_LOSS_BPR) {
-            l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-            g = -1.0f / (1.0f + expf(x));
-        } else if (loss_kind == NRC_LOSS_HINGE) {
-            const float t = x + 1.0f; l = fmaxf(t, 0.f); g = (t > 0.f) ? 1.f : 0.f;
-        } else {
-            const float t = 1.0f - x; l = t * t; g = -2.0f * t;
-        }
-    } else {
-        const float x = yhat[0], z = reinterpret_cast<const float*>(third)[b];
-        if (loss_kind == NRC_LOSS_CROSS_ENTROPY) {
-            const float inv_b = 1.0f / (float)batch;
-            const float e = expf(-fabsf(x));
-            l = (fmaxf(x, 0.f) - x * z + log1pf(e)) * inv_b;
-            const float s = (x >= 0.f) ? 1.f / (1.f + e) : e / (1.f + e);
-            g = (s - z) * inv_b;
-        } else {
-            const float t = z - x; l = t * t; g = -2.0f * t;
-        }
-    }
+    if (pairwise)   // NeuMF.py:92 result = output - output_neg
+        pairwise_loss_grad(loss_kind, yhat[0] - yhat[1], l, g);
+    else
+        pointwise_loss_grad(loss_kind, yhat[0], reinterpret_cast<const float*>(third)[b], 1.0f / (float)batch, l, g);
 
     float sq_mf = 0.f, sq_mlp = 0.f;
     for (int p = 0; p < passes; ++p) {
@@ -304,28 +287,8 @@ ncf_sample_fast_kernel(const NcfDev S, const NcfPtrs P, const int32_t* __restric
     }
 
     float l, g;
-    if (pairwise) {
-        const float x = yhat[0] - yhat[1];
-        if (loss_kind == NRC_LOSS_BPR) {
-            l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-            g = -1.0f / (1.0f + expf(x));
-        } else if (loss_kind == NRC_LOSS_HINGE) {
-            const float t = x + 1.0f; l = fmaxf(t, 0.f); g = (t > 0.f) ? 1.f : 0.f;
-        } else {
-            const float t = 1.0f - x; l = t * t; g = -2.0f * t;
-        }
-    } else {
-        const float x = yhat[0], z = reinterpret_cast<const float*>(third)[b];
-        if (loss_kind == NRC_LOSS_CROSS_ENTROPY) {
-            const float inv_b = 1.0f / (float)batch;
-            const float e = expf(-fabsf(x));
-            l = (fmaxf(x, 0.f) - x * z + log1pf(e)) * inv_b;
-            const float s = (x >= 0.f) ? 1.f / (1.f + e) : e / (1.f + e);
-            g = (s - z) * inv_b;
-        } else {
-            const float t = z - x; l = t * t; g = -2.0f * t;
-        }
-    }
+    if (pairwise) pairwise_loss_grad(loss_kind, yhat[0] - yhat[1], l, g);
+    else pointwise_loss_grad(loss_kind, yhat[0], reinterpret_cast<const float*>(third)[b], 1.0f / (float)batch, l, g);
 
     float sq_mf = 0.f, sq_mlp = 0.f;
     for (int p = 0; p < passes; ++p) {

@@ -22,9 +22,8 @@
 //   grid barrier.
 // Arithmetic identical to nrc_ncf_train_epoch except for the summation order of dW (fixed slices
 // instead of atomics) -- tests compare both with oracle/tf_math.NCFTrainer.
-#include <stdlib.h>
-
 #include "epoch.cuh"
+#include "learner.cuh"
 #include "ncf.cuh"
 #include "optim.cuh"
 
@@ -52,10 +51,9 @@ struct NcfEpochParams {
     float* adam_pows;
     unsigned int* barrier;
     int64_t n_used, first_step, num_steps, steps_total;
-    int32_t batch_size, pairwise, loss_kind, opt_kind, first_stamp, build, bar_mode;
+    int32_t batch_size, pairwise, loss_kind, opt_kind, first_stamp, build;
     int64_t seg_end[4];                    // running float4-group counts of seg[0..3] (tables_vec4)
     int32_t tables_vec4;                   // every table width a multiple of 4 (and 16-byte aligned rows)
-    int32_t dbg;                           // NRC_EPOCH_DBG bits (0 in normal use): 1 skip samples, 2 skip weight gradients, 4 skip tables, 8 skip weight staging
     int32_t sw_floats;                     // shared-memory floats of the weight copy (towers, rounded up to 4)
     int32_t wblocked, wblocks, sred_off;   // blocked weight-gradient path: 4 x 4 blocks per tower; smem offset (floats) of its reduction slots
     float reg_mf, reg_mlp, h0, h1, h2, h3;
@@ -154,28 +152,8 @@ __device__ __forceinline__ void ncf_sample(const NcfEpochParams& Q, const float*
         yhat[p] = group_sum(mf + s, red, tid, grp);      // NeuMF.py:85 reduce_sum(concat(mf, mlp))
     }
     float l, g;
-    if (Q.pairwise) {
-        const float x = yhat[0] - yhat[1];               // NeuMF.py:92
-        if (Q.loss_kind == NRC_LOSS_BPR) {
-            l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-            g = -1.0f / (1.0f + expf(x));
-        } else if (Q.loss_kind == NRC_LOSS_HINGE) {
-            const float t = x + 1.0f; l = fmaxf(t, 0.f); g = (t > 0.f) ? 1.f : 0.f;
-        } else {
-            const float t = 1.0f - x; l = t * t; g = -2.0f * t;
-        }
-    } else {
-        const float x = yhat[0], z = __int_as_float(third);
-        if (Q.loss_kind == NRC_LOSS_CROSS_ENTROPY) {
-            const float inv_b = 1.0f / (float)cnt;
-            const float e = expf(-fabsf(x));
-            l = (fmaxf(x, 0.f) - x * z + log1pf(e)) * inv_b;
-            const float s = (x >= 0.f) ? 1.f / (1.f + e) : e / (1.f + e);
-            g = (s - z) * inv_b;
-        } else {
-            const float t = z - x; l = t * t; g = -2.0f * t;
-        }
-    }
+    if (Q.pairwise) pairwise_loss_grad(Q.loss_kind, yhat[0] - yhat[1], l, g);   // NeuMF.py:92
+    else pointwise_loss_grad(Q.loss_kind, yhat[0], __int_as_float(third), 1.0f / (float)cnt, l, g);
     float sq_mf = 0.f, sq_mlp = 0.f;
     for (int p = 0; p < passes; ++p) {
         const float gp = (p == 0) ? g : -g;
@@ -243,7 +221,7 @@ __global__ void __launch_bounds__(kEpThreads, 1) ncf_epoch_kernel(const NcfEpoch
             Q.ws_u[p] = u; Q.ws_i[p] = it; Q.ws_t[p] = th;
         }
         for (int64_t s = gtid; s < Q.steps_total; s += nthr) Q.step_loss[s] = 0.0f;
-        grid_barrier(Q.barrier, target, Q.bar_mode);
+        grid_barrier(Q.barrier, target);
     }
     const bool adam = Q.opt_kind == NRC_OPT_ADAM;
     float p1 = 0.0f, p2 = 0.0f;
@@ -258,7 +236,7 @@ __global__ void __launch_bounds__(kEpThreads, 1) ncf_epoch_kernel(const NcfEpoch
         const int64_t cnt = (Q.n_used - off < Q.batch_size) ? (Q.n_used - off) : Q.batch_size;
         const int32_t stamp = Q.first_stamp + (int32_t)(s - Q.first_step);
         // ---- phase 1: this step's weights -> shared memory (padded rows), then the samples
-        if (!(Q.dbg & 8)) {   // straight float4 copy (the packed dense buffer is 16-byte aligned and sw_floats is a multiple of 4):
+        {   // straight float4 copy (the packed dense buffer is 16-byte aligned and sw_floats is a multiple of 4):
             // every thread's loads are independent -> one L2 round trip
             const int n4 = Q.sw_floats >> 2, total = S.tower_size * S.n_towers;
             const float4* src4 = reinterpret_cast<const float4*>(Q.dense);
@@ -288,14 +266,14 @@ __global__ void __launch_bounds__(kEpThreads, 1) ncf_epoch_kernel(const NcfEpoch
         }
         __syncthreads();
         float loss_acc = 0.0f;
-        for (int64_t b = (int64_t)blockIdx.x * kGroups + grp; b < cnt && !(Q.dbg & 1); b += (int64_t)gridDim.x * kGroups) {
+        for (int64_t b = (int64_t)blockIdx.x * kGroups + grp; b < cnt; b += (int64_t)gridDim.x * kGroups) {
             float l = 0.0f;
             ncf_sample(Q, sW, sAct, sDel, part, red, tid, grp, b, cnt, __ldcg(Q.ws_u + off + b), __ldcg(Q.ws_i + off + b),
                        __ldcg(Q.ws_t + off + b), stamp, l);
             loss_acc += l;
         }
         if (tid == 0 && loss_acc != 0.0f) atomicAdd(Q.step_loss + s, loss_acc);
-        grid_barrier(Q.barrier, target, Q.bar_mode);
+        grid_barrier(Q.barrier, target);
         // ---- phase 2
         float h0 = Q.h0;
         if (adam) {
@@ -308,8 +286,7 @@ __global__ void __launch_bounds__(kEpThreads, 1) ncf_epoch_kernel(const NcfEpoch
         // lane64 + 64, ... with ONE float4 of activations and ONE float4 of deltas per sample (all loads of a
         // thread are independent: one L2 round trip), 16 FMAs per sample; the 64 partial blocks are summed by
         // warp shuffles + one shared-memory hop in fixed order; 16 lanes apply the dense optimizer formula.
-        if (Q.dbg & 2) {
-        } else if (Q.wblocked) {
+        if (Q.wblocked) {
             const int grp64 = tid_cta >> 6, l64 = tid_cta & 63, wl = tid_cta & 31;
             float* sred = sm + Q.sred_off + grp64 * 16;
             for (int bi = blockIdx.x * (kEpThreads / 64) + grp64; bi < Q.wblocks * S.n_towers; bi += gridDim.x * (kEpThreads / 64)) {
@@ -413,8 +390,7 @@ __global__ void __launch_bounds__(kEpThreads, 1) ncf_epoch_kernel(const NcfEpoch
         }
         // (b) embedding tables.  All four tables form ONE flat space of float4 groups (a grid of one 256-thread
         // CTA per SM covers ml-100k's 26k groups in a single trip: one latency chain instead of four).
-        if (Q.dbg & 4) {
-        } else if (Q.tables_vec4) {
+        if (Q.tables_vec4) {
             const bool stamped = !(adam || Q.opt_kind == NRC_OPT_GD);
             const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
             for (int64_t gi = gtid; gi < Q.seg_end[3]; gi += nthr) {
@@ -452,7 +428,7 @@ __global__ void __launch_bounds__(kEpThreads, 1) ncf_epoch_kernel(const NcfEpoch
                 }
             }
         }
-        grid_barrier(Q.barrier, target, Q.bar_mode);
+        grid_barrier(Q.barrier, target);
     }
     if (adam && gtid == 0) { Q.adam_pows[0] = p1; Q.adam_pows[1] = p2; }
 }
@@ -545,12 +521,7 @@ extern "C" int nrc_ncf_epoch_fused(const nrc_ncf_shape* shape, float* mf_user, f
     Q.scratch = g_ep_scratch; Q.step_loss = step_loss; Q.adam_pows = adam_pows;
     Q.first_step = first_step; Q.num_steps = num_steps;
     Q.batch_size = batch_size; Q.pairwise = pairwise ? 1 : 0; Q.loss_kind = loss_kind; Q.opt_kind = opt_kind;
-    Q.first_stamp = first_stamp; Q.build = first_step == 0 ? 1 : 0; Q.bar_mode = epoch_bar_mode();
-    {
-        static int dbg = -1;
-        if (dbg < 0) { const char* e = getenv("NRC_EPOCH_DBG"); dbg = e ? atoi(e) : 0; }
-        Q.dbg = dbg;
-    }
+    Q.first_stamp = first_stamp; Q.build = first_step == 0 ? 1 : 0;
     Q.reg_mf = reg_mf; Q.reg_mlp = reg_mlp;
     Q.h0 = hyper_host ? hyper_host[0] : 0.0f; Q.h1 = hyper_host ? hyper_host[1] : 0.0f;
     Q.h2 = hyper_host ? hyper_host[2] : 0.0f; Q.h3 = hyper_host ? hyper_host[3] : 0.0f;

@@ -25,6 +25,7 @@
 //                           one RED per weight entry and CTA at the end
 //   the remaining A_hat^T . dside is nrc_spmm_csr with its fused bias (dego + A^T dside).
 #include "common.cuh"
+#include "learner.cuh"
 #include "philox.cuh"
 
 namespace nrc {
@@ -160,9 +161,9 @@ ngcf_bpr_grad_kernel(const float* __restrict__ E, int D, int num_users, const in
         }
         di = warp_sum(di); dj = warp_sum(dj); sq = warp_sum(sq);
         const float x = di - dj;
-        mf_acc += (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));     // softplus(-x)
+        mf_acc += neg_log_sigmoid(x);     // softplus(-x)
         emb_acc += reg * 0.5f * sq;
-        const float g = -1.0f / (1.0f + expf(x));
+        const float g = neg_log_sigmoid_grad(x);
         for (int k = lane; k < D; k += kWarp) {
             const float a = E[ru + k], bi = E[ri + k], bj = E[rj + k];
             atomicAdd(G + ru + k, g * (bi - bj) + reg * a);

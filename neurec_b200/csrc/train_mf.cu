@@ -20,130 +20,28 @@
 
 #include "common.cuh"
 #include "epoch.cuh"
+#include "learner.cuh"
+#include "mf.cuh"
 #include "optim.cuh"
 
 namespace nrc {
 
-// softplus(-x) = -log_sigmoid(x)  (learner.py:22, tool.py:224)
-__device__ __forceinline__ float neg_log_sigmoid(float x) {
-    return (x >= 0.0f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-}
-
-// d/dx of the pairwise loss l(x)
-__device__ __forceinline__ void pairwise_loss_grad(int kind, float x, float& l, float& g) {
-    if (kind == NRC_LOSS_BPR) {           // learner.py:21-22  -sum(log_sigmoid(y))
-        l = neg_log_sigmoid(x);
-        g = -1.0f / (1.0f + expf(x));     // -sigmoid(-x)
-    } else if (kind == NRC_LOSS_HINGE) {  // learner.py:23-24  sum(max(y + margin, 0)) [sic]
-        const float t = x + 1.0f;
-        l = fmaxf(t, 0.0f);
-        g = (t > 0.0f) ? 1.0f : 0.0f;
-    } else {                              // learner.py:25-26  sum((1 - y)^2)
-        const float t = 1.0f - x;
-        l = t * t;
-        g = -2.0f * t;
-    }
-}
-
+// Phase 1 of a step: one warp per triplet (PAIRWISE: third = negative items) or sample (third = labels' bits).
+// The any-dim form of mf_sample_grad, ordinary loads.
+template <bool PAIRWISE>
 __global__ void __launch_bounds__(256)
-mf_pairwise_grad_kernel(const float* __restrict__ U, const float* __restrict__ V, int D,
-                        const int32_t* __restrict__ users, const int32_t* __restrict__ pos,
-                        const int32_t* __restrict__ neg, int64_t batch, int loss_kind, float reg,
-                        float* __restrict__ gU, float* __restrict__ gV,
-                        int32_t* __restrict__ tU, int32_t* __restrict__ tV, int32_t stamp,
-                        float* __restrict__ loss) {
-    const int lane = threadIdx.x & 31;
-    const int wib = threadIdx.x >> 5;
-    const int wpb = blockDim.x >> 5;
-    float loss_acc = 0.0f;
-    for (int64_t b = (int64_t)blockIdx.x * wpb + wib; b < batch; b += (int64_t)gridDim.x * wpb) {
-        const int u = users[b], i = pos[b], j = neg[b];
-        const float* __restrict__ pu = U + (size_t)u * D;
-        const float* __restrict__ qi = V + (size_t)i * D;
-        const float* __restrict__ qj = V + (size_t)j * D;
-        float di = 0.0f, dj = 0.0f, sq = 0.0f;
-        for (int k = lane; k < D; k += kWarp) {
-            const float a = pu[k], bi = qi[k], bj = qj[k];
-            di = fmaf(a, bi, di);
-            dj = fmaf(a, bj, dj);
-            sq += a * a + bi * bi + bj * bj;
-        }
-        di = warp_sum(di);
-        dj = warp_sum(dj);
-        const float x = di - dj;  // MF.py:66  result = output - output_neg
-        float l, g;
-        pairwise_loss_grad(loss_kind, x, l, g);
-        if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);  // MF.py:67 reg * l2_loss(p1, q2, q1)
-        loss_acc += l;
-        float* gu = gU + (size_t)u * D;
-        float* gi = gV + (size_t)i * D;
-        float* gj = gV + (size_t)j * D;
-        for (int k = lane; k < D; k += kWarp) {
-            const float a = pu[k], bi = qi[k], bj = qj[k];
-            atomicAdd(gu + k, g * (bi - bj) + reg * a);
-            atomicAdd(gi + k, g * a + reg * bi);
-            atomicAdd(gj + k, -g * a + reg * bj);
-        }
-        if (lane == 0) {
-            tU[u] = stamp;
-            tV[i] = stamp;
-            tV[j] = stamp;
-        }
-    }
-    if (lane == 0 && loss) atomicAdd(loss, loss_acc);
-}
-
-__global__ void __launch_bounds__(256)
-mf_pointwise_grad_kernel(const float* __restrict__ U, const float* __restrict__ V, int D,
-                         const int32_t* __restrict__ users, const int32_t* __restrict__ items,
-                         const float* __restrict__ labels, int64_t batch, int loss_kind, float reg,
-                         float* __restrict__ gU, float* __restrict__ gV,
-                         int32_t* __restrict__ tU, int32_t* __restrict__ tV, int32_t stamp,
-                         float* __restrict__ loss) {
+mf_grad_kernel(const float* __restrict__ U, const float* __restrict__ V, int D, const int32_t* __restrict__ users,
+               const int32_t* __restrict__ items, const int32_t* __restrict__ third, int64_t batch, int loss_kind,
+               float reg, float* __restrict__ gU, float* __restrict__ gV, int32_t* __restrict__ tU,
+               int32_t* __restrict__ tV, int32_t stamp, float* __restrict__ loss) {
     const int lane = threadIdx.x & 31;
     const int wib = threadIdx.x >> 5;
     const int wpb = blockDim.x >> 5;
     const float inv_b = 1.0f / (float)batch;
     float loss_acc = 0.0f;
-    for (int64_t b = (int64_t)blockIdx.x * wpb + wib; b < batch; b += (int64_t)gridDim.x * wpb) {
-        const int u = users[b], i = items[b];
-        const float z = labels[b];
-        const float* __restrict__ pu = U + (size_t)u * D;
-        const float* __restrict__ qi = V + (size_t)i * D;
-        float x = 0.0f, sq = 0.0f;
-        for (int k = lane; k < D; k += kWarp) {
-            const float a = pu[k], bi = qi[k];
-            x = fmaf(a, bi, x);
-            sq += a * a + bi * bi;
-        }
-        x = warp_sum(x);
-        float l, g;
-        if (loss_kind == NRC_LOSS_CROSS_ENTROPY) {
-            // learner.py:33-34 tf.losses.sigmoid_cross_entropy: mean_b of
-            // max(x,0) - x*z + log1p(exp(-|x|))
-            const float e = expf(-fabsf(x));
-            l = (fmaxf(x, 0.0f) - x * z + log1pf(e)) * inv_b;
-            const float s = (x >= 0.0f) ? 1.0f / (1.0f + e) : e / (1.0f + e);
-            g = (s - z) * inv_b;
-        } else {  // learner.py:37-38 sum((y_rea - y_pre)^2)
-            const float t = z - x;
-            l = t * t;
-            g = -2.0f * t;
-        }
-        if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);  // MF.py:72 reg * l2_loss(p1, q1)
-        loss_acc += l;
-        float* gu = gU + (size_t)u * D;
-        float* gi = gV + (size_t)i * D;
-        for (int k = lane; k < D; k += kWarp) {
-            const float a = pu[k], bi = qi[k];
-            atomicAdd(gu + k, g * bi + reg * a);
-            atomicAdd(gi + k, g * a + reg * bi);
-        }
-        if (lane == 0) {
-            tU[u] = stamp;
-            tV[i] = stamp;
-        }
-    }
+    for (int64_t b = (int64_t)blockIdx.x * wpb + wib; b < batch; b += (int64_t)gridDim.x * wpb)
+        loss_acc += mf_sample_grad<PAIRWISE, 0, false>(U, V, gU, gV, tU, tV, D, reg, loss_kind, lane, users[b], items[b],
+                                                       third[b], inv_b, stamp);
     if (lane == 0 && loss) atomicAdd(loss, loss_acc);
 }
 
@@ -215,9 +113,7 @@ __device__ __forceinline__ void red_row(float* p, const float (&d)[VEC], bool re
         for (int t = 0; t < VEC; ++t) atomicAdd(p + t, d[t]);
         return;
     }
-    if constexpr (VEC == 4) atomicAdd(reinterpret_cast<float4*>(p), make_float4(d[0], d[1], d[2], d[3]));
-    else if constexpr (VEC == 2) atomicAdd(reinterpret_cast<float2*>(p), make_float2(d[0], d[1]));
-    else atomicAdd(p, d[0]);
+    red_vec<VEC>(p, d);
 }
 
 template <int VEC, bool SHARDED>
@@ -235,19 +131,7 @@ mf_bpr_sgd_fused_kernel(const RowShards U, const RowShards V, const int32_t* __r
         float* qi = V.row<SHARDED>(pos[b], D, ri) + lane * VEC;
         float* qj = V.row<SHARDED>(neg[b], D, rj) + lane * VEC;
         float a[VEC], bi[VEC], bj[VEC];
-        if constexpr (VEC == 4) {
-            const float4 x = *reinterpret_cast<const float4*>(pu), y = *reinterpret_cast<const float4*>(qi),
-                         z = *reinterpret_cast<const float4*>(qj);
-            a[0] = x.x; a[1] = x.y; a[2] = x.z; a[3] = x.w;
-            bi[0] = y.x; bi[1] = y.y; bi[2] = y.z; bi[3] = y.w;
-            bj[0] = z.x; bj[1] = z.y; bj[2] = z.z; bj[3] = z.w;
-        } else if constexpr (VEC == 2) {
-            const float2 x = *reinterpret_cast<const float2*>(pu), y = *reinterpret_cast<const float2*>(qi),
-                         z = *reinterpret_cast<const float2*>(qj);
-            a[0] = x.x; a[1] = x.y; bi[0] = y.x; bi[1] = y.y; bj[0] = z.x; bj[1] = z.y;
-        } else {
-            a[0] = *pu; bi[0] = *qi; bj[0] = *qj;
-        }
+        ld_vec<VEC>(pu, a); ld_vec<VEC>(qi, bi); ld_vec<VEC>(qj, bj);
         float di = 0.f, dj = 0.f, sq = 0.f;
 #pragma unroll
         for (int t = 0; t < VEC; ++t) {
@@ -257,10 +141,10 @@ mf_bpr_sgd_fused_kernel(const RowShards U, const RowShards V, const int32_t* __r
         }
         di = warp_sum(di); dj = warp_sum(dj);
         const float x = di - dj;
-        float l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
+        float l = neg_log_sigmoid(x);
         if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);
         loss_acc += l;
-        const float g = -1.0f / (1.0f + expf(x));
+        const float g = neg_log_sigmoid_grad(x);
         float du[VEC], dvi[VEC], dvj[VEC];
 #pragma unroll
         for (int t = 0; t < VEC; ++t) {
@@ -314,25 +198,6 @@ static int launch_bpr_sgd(const RowShards& SU, const RowShards& SV, int dim, con
 // User rows are always local (the train CSR is sharded by user owner, SURVEY 8e); item rows may
 // live on any rank (RowShards) and are then read / RED-updated over NVLink by the same kernel.
 // ----------------------------------------------------------------------------------------
-template <int VEC>
-__device__ __forceinline__ void ld_vec(const float* p, float (&v)[VEC]) {
-    if constexpr (VEC == 4) {
-        const float4 x = *reinterpret_cast<const float4*>(p);
-        v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
-    } else if constexpr (VEC == 2) {
-        const float2 x = *reinterpret_cast<const float2*>(p);
-        v[0] = x.x; v[1] = x.y;
-    } else {
-        v[0] = *p;
-    }
-}
-
-template <int VEC>
-__device__ __forceinline__ void st_vec(float* p, const float (&v)[VEC]) {
-    if constexpr (VEC == 4) *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-    else if constexpr (VEC == 2) *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
-    else *p = v[0];
-}
 
 // Rows [0, T) of the replicated head are held in shared memory for the whole launch, T = 32 KB of rows (64 at
 // d = 128).  They are the most popular items: at the benchmark's Zipf(1.05) law the top 64 take ~11 % of all row
@@ -426,10 +291,10 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
                 if (t0 + k >= n) break;
                 const int t = t0 + k;
                 const float x = di[k] - dj[k];
-                float l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
+                float l = neg_log_sigmoid(x);
                 if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq[k]);
                 loss_acc += l;
-                const float g = -1.0f / (1.0f + expf(x));
+                const float g = neg_log_sigmoid_grad(x);
                 float du[VEC], dvi[VEC], dvj[VEC];
 #pragma unroll
                 for (int q = 0; q < VEC; ++q) {
@@ -457,181 +322,6 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
     if (lane == 0 && loss) atomicAdd(loss, loss_acc);
 }
 
-// ----------------------------------------------------------------------------------------
-// Pipelined form of the CSR-fed step (NRC_SGD_PIPE=1 / nrc_mf_sgd_set_pipelined; NOT the default, which is the
-// register form above.  The alternative north_star names: rows staged through shared memory by the bulk-copy engine).
-// The register form keeps 2 triplets per warp in flight and alternates a sampling phase with an update phase;
-// it is latency-bound (dependent row gathers and RED round trips).  Here the rows never
-// pass through registers on their way in or out, and sampling runs ahead of the row traffic:
-//   samplers (16 warps, 512 threads): bijection -> (user, positive) -> rejection draw; the ids go into a
-//       512-entry shared-memory queue (sequence-numbered entries, one per sampler thread).  A sampling chain is
-//       4-5 DEPENDENT DRAM round trips, so throughput = chains in flight / chain latency: 512 per SM.
-//   consumers (8 warps, 16 ring slots each): lane 0 takes the next ids from the queue and issues three bulk copies
-//       (cp.async.bulk, one row each) into the slot, completion counted on the slot's mbarrier; when the rows
-//       have landed the warp reads them into registers, REFILLS THE SLOT AT ONCE with its next triplet, and
-//       finishes the current one out of registers: dots by shuffle, deltas by vector RED.ADD (local and peer
-//       rows alike).  (Returning the deltas through the copy engine as bulk reduce-adds -- the first version --
-//       keeps a slot busy until the engine has read them back.)
-// 128 slots x 3 rows in flight per SM (192 KB at d = 128) whatever the register pressure.  One CTA per SM.
-// CTA-local sequence number n <-> ring slot n % 128, round n / 128, position first + blockIdx*128 + slot + round*stride.
-// ----------------------------------------------------------------------------------------
-constexpr int kPipeSlots = 128, kPipeSamplerWarps = 16, kPipeConsWarps = 8;
-constexpr int kPipeSamplers = kPipeSamplerWarps * 32;          // = id-queue entries (one per sampler thread)
-constexpr int kPipeThreads = (kPipeSamplerWarps + kPipeConsWarps) * 32;
-
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    while (!done)
-        asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-}
-
-struct PipeIds { int32_t u, i, j, pad; };
-
-template <int VEC, bool SHARDED>
-__global__ void __launch_bounds__(kPipeThreads, 1)
-mf_bpr_sgd_pipe_kernel(float* __restrict__ U_local, const RowShards V, const EpochSpec E, int64_t first,
-                       int64_t count, float lr, float reg, float* __restrict__ loss) {
-    constexpr int D = 32 * VEC;
-    constexpr uint32_t kRowBytes = D * 4;
-    extern __shared__ __align__(128) unsigned char pipe_smem[];
-    float* ring = reinterpret_cast<float*>(pipe_smem);                              // [slots][3][D]
-    uint64_t* full = reinterpret_cast<uint64_t*>(pipe_smem + (size_t)kPipeSlots * 3 * kRowBytes);   // [slots]
-    PipeIds* idq = reinterpret_cast<PipeIds*>(full + kPipeSlots);                   // [samplers]
-    volatile int32_t* seq_ready = reinterpret_cast<volatile int32_t*>(idq + kPipeSamplers);   // n + 1 once entry n % Q is filled
-    volatile int32_t* seq_done = seq_ready + kPipeSamplers;                         // n + 1 once it has been taken
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < kPipeSlots) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((uint32_t)__cvta_generic_to_shared(full + tid)));
-    for (int e = tid; e < kPipeSamplers; e += kPipeThreads) { seq_ready[e] = 0; seq_done[e] = 0; }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncthreads();
-    const int64_t stride = (int64_t)gridDim.x * kPipeSlots;
-    const int64_t base = (int64_t)blockIdx.x * kPipeSlots;
-    // rounds this CTA takes part in, and its sequence numbers [0, n_end); entries whose position is past `count`
-    // (the ragged last round) are skipped by samplers and consumers alike
-    const int64_t rounds = (count > base) ? (count - base + stride - 1) / stride : 0;
-    const int32_t n_end = (int32_t)(rounds * kPipeSlots);
-    auto pos_of = [&](int32_t n) { return base + (n % kPipeSlots) + (int64_t)(n / kPipeSlots) * stride; };
-    if (warp < kPipeSamplerWarps) {
-        for (int32_t n = tid; n < n_end; n += kPipeSamplers) {
-            const int64_t q = pos_of(n);
-            if (q >= count) continue;
-            int32_t u, i, j;
-            epoch_sample(E, first + q, 0, u, i, j);
-            if (n >= kPipeSamplers) {                       // this thread's previous entry must have been taken
-                const int32_t want = n - kPipeSamplers + 1;
-                while (seq_done[tid] != want) __nanosleep(256);     // samplers run ahead: sleep, do not steal issue slots from the consumers
-            }
-            idq[tid] = PipeIds{u, i, j, 0};
-            __threadfence_block();
-            seq_ready[tid] = n + 1;
-        }
-    } else {
-        const int cw = warp - kPipeSamplerWarps;
-        float loss_acc = 0.0f;
-        // the update addresses of the triplet in each of this warp's 16 slots (lane k keeps slot cw + 8k)
-        float *upd_u = nullptr, *upd_i = nullptr, *upd_j = nullptr;
-        auto load_slot = [&](int32_t n) {                  // whole warp; lane 0 works, lane (slot index) remembers
-            const int s = n % kPipeSlots, e = n % kPipeSamplers, k = s / kPipeConsWarps;
-            float *pu = nullptr, *wi = nullptr, *wj = nullptr;
-            if (lane == 0) {
-                while (seq_ready[e] != n + 1) __nanosleep(64);
-                __threadfence_block();
-                const PipeIds t = idq[e];
-                __threadfence_block();
-                seq_done[e] = n + 1;
-                bool ri, rj;
-                pu = U_local + (size_t)t.u * D;
-                float* qi = V.row<SHARDED>(t.i, D, ri, wi);
-                float* qj = V.row<SHARDED>(t.j, D, rj, wj);
-                const uint32_t bar = (uint32_t)__cvta_generic_to_shared(full + s);
-                const uint32_t dst = (uint32_t)__cvta_generic_to_shared(ring + (size_t)s * 3 * D);
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(3 * kRowBytes) : "memory");
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(dst), "l"(pu), "r"(kRowBytes), "r"(bar) : "memory");
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(dst + kRowBytes), "l"(qi), "r"(kRowBytes), "r"(bar) : "memory");
-                asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                             ::"r"(dst + 2 * kRowBytes), "l"(qj), "r"(kRowBytes), "r"(bar) : "memory");
-            }
-            pu = reinterpret_cast<float*>(__shfl_sync(kFull, (unsigned long long)pu, 0));
-            wi = reinterpret_cast<float*>(__shfl_sync(kFull, (unsigned long long)wi, 0));
-            wj = reinterpret_cast<float*>(__shfl_sync(kFull, (unsigned long long)wj, 0));
-            if (lane == k) { upd_u = pu; upd_i = wi; upd_j = wj; }
-        };
-        constexpr int kMine = kPipeSlots / kPipeConsWarps;         // 16 slots per consumer warp
-        // prologue: round 0 of every slot of this warp
-        for (int k = 0; k < kMine; ++k) {
-            const int32_t n = cw + k * kPipeConsWarps;
-            if (n < n_end && pos_of(n) < count) load_slot(n);
-        }
-        for (int32_t r = 0; r < (int32_t)rounds; ++r) {
-            for (int k = 0; k < kMine; ++k) {
-                const int s = cw + k * kPipeConsWarps;
-                const int32_t n = r * kPipeSlots + s;
-                if (pos_of(n) >= count) continue;
-                mbar_wait((uint32_t)__cvta_generic_to_shared(full + s), r & 1);
-                float* slot = ring + (size_t)s * 3 * D + lane * VEC;
-                float a[VEC], bi[VEC], bj[VEC];
-                ld_vec<VEC>(slot, a); ld_vec<VEC>(slot + D, bi); ld_vec<VEC>(slot + 2 * D, bj);
-                float di = 0.f, dj = 0.f, sq = 0.f;
-#pragma unroll
-                for (int t = 0; t < VEC; ++t) {
-                    di = fmaf(a[t], bi[t], di); dj = fmaf(a[t], bj[t], dj);
-                    sq += a[t] * a[t] + bi[t] * bi[t] + bj[t] * bj[t];
-                }
-                di = warp_sum(di); dj = warp_sum(dj);      // every lane's row reads have completed (the sums depend on them)
-                // where this triplet's deltas go, then refill the slot at once: the rows are in registers now
-                float* const p0 = reinterpret_cast<float*>(__shfl_sync(kFull, (unsigned long long)upd_u, k)) + lane * VEC;
-                float* const p1 = reinterpret_cast<float*>(__shfl_sync(kFull, (unsigned long long)upd_i, k)) + lane * VEC;
-                float* const p2 = reinterpret_cast<float*>(__shfl_sync(kFull, (unsigned long long)upd_j, k)) + lane * VEC;
-                {
-                    const int32_t nn = n + kPipeSlots;                   // same slot, next round
-                    if (nn < n_end && pos_of(nn) < count) load_slot(nn);
-                }
-                const float x = di - dj;
-                float l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
-                if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);
-                loss_acc += l;
-                const float g = -1.0f / (1.0f + expf(x));
-                float du[VEC], dvi[VEC], dvj[VEC];
-#pragma unroll
-                for (int t = 0; t < VEC; ++t) {
-                    du[t] = -lr * (g * (bi[t] - bj[t]) + reg * a[t]);
-                    dvi[t] = -lr * (g * a[t] + reg * bi[t]);
-                    dvj[t] = -lr * (-g * a[t] + reg * bj[t]);
-                }
-                red_row<VEC>(p0, du, false);       // vector REDs, local and peer rows alike
-                red_row<VEC>(p1, dvi, false);
-                red_row<VEC>(p2, dvj, false);
-            }
-        }
-        if (lane == 0 && loss) atomicAdd(loss, loss_acc);
-    }
-}
-
-template <int VEC, bool SH>
-static int launch_pipe(float* U_local, const RowShards& SV, const EpochSpec& E, int64_t first, int64_t count, float lr,
-                       float reg, float* loss, cudaStream_t st) {
-    constexpr size_t smem = (size_t)kPipeSlots * 3 * (32 * VEC * 4) + (size_t)kPipeSlots * 8 + (size_t)kPipeSamplers * (16 + 8);
-    static bool attr = false;
-    if (!attr) {
-        NRC_CUDA_CHECK(cudaFuncSetAttribute(mf_bpr_sgd_pipe_kernel<VEC, SH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = true;
-    }
-    int64_t blocks = (count + kPipeSlots - 1) / kPipeSlots;
-    if (blocks > sm_count()) blocks = sm_count();
-    mf_bpr_sgd_pipe_kernel<VEC, SH><<<(unsigned)blocks, kPipeThreads, smem, st>>>(U_local, SV, E, first, count, lr, reg, loss);
-    NRC_CUDA_CHECK(cudaGetLastError());
-    return NRC_OK;
-}
-
-static int g_sgd_pipe = -1;
-static int sgd_pipe_enabled() {
-    if (g_sgd_pipe < 0) { const char* e = getenv("NRC_SGD_PIPE"); g_sgd_pipe = e ? (atoi(e) != 0) : 0; }
-    return g_sgd_pipe;
-}
-
 template <int VEC, bool SH>
 static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E, int64_t first, int64_t count, float lr,
                          float reg, float* loss, cudaStream_t st) {
@@ -655,12 +345,6 @@ static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E
 static int launch_bpr_sgd_stream(float* U_local, const RowShards& SV, int dim, const EpochSpec& E, int64_t first,
                                  int64_t count, float lr, float reg, float* loss, cudaStream_t st) {
     const bool sharded = SV.rows_per_shard != 0;
-    if (sgd_pipe_enabled() && !SV.force_remote && (dim == 128 || dim == 64)) {
-        if (dim == 128) return sharded ? launch_pipe<4, true>(U_local, SV, E, first, count, lr, reg, loss, st)
-                                       : launch_pipe<4, false>(U_local, SV, E, first, count, lr, reg, loss, st);
-        return sharded ? launch_pipe<2, true>(U_local, SV, E, first, count, lr, reg, loss, st)
-                       : launch_pipe<2, false>(U_local, SV, E, first, count, lr, reg, loss, st);
-    }
 #define NRC_STREAM(VEC) (sharded ? launch_stream<VEC, true>(U_local, SV, E, first, count, lr, reg, loss, st) \
                                  : launch_stream<VEC, false>(U_local, SV, E, first, count, lr, reg, loss, st))
     if (dim == 128) return NRC_STREAM(4);
@@ -729,10 +413,10 @@ mf_bpr_lazy_adam_stream_kernel(float* __restrict__ U, float* __restrict__ mU, fl
             }
             di = warp_sum(di); dj = warp_sum(dj);
             const float x = di - dj;
-            float l = (x >= 0.f) ? log1pf(expf(-x)) : (-x + log1pf(expf(x)));
+            float l = neg_log_sigmoid(x);
             if (reg != 0.0f) l += reg * 0.5f * warp_sum(sq);
             loss_acc += l;
-            const float g = -1.0f / (1.0f + expf(x));
+            const float g = neg_log_sigmoid_grad(x);
             float gu[VEC], gi[VEC], gj[VEC];
 #pragma unroll
             for (int c = 0; c < VEC; ++c) {
@@ -774,7 +458,7 @@ extern "C" int nrc_mf_pairwise_grad(const float* user_table, const float* item_t
                 NRC_E_VALUE, "please choose a suitable loss function");
     NRC_REQUIRE(dim > 0 && batch >= 0, NRC_E_VALUE, "dim must be positive, batch >= 0");
     if (batch == 0) return NRC_OK;
-    mf_pairwise_grad_kernel<<<grad_grid(batch), 256, 0, as_stream(stream)>>>(
+    mf_grad_kernel<true><<<grad_grid(batch), 256, 0, as_stream(stream)>>>(
         user_table, item_table, dim, users, pos_items, neg_items, batch, loss_kind, reg, grad_user,
         grad_item, touched_user, touched_item, stamp, loss);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -792,9 +476,9 @@ extern "C" int nrc_mf_pointwise_grad(const float* user_table, const float* item_
                 "please choose a suitable loss function");
     NRC_REQUIRE(dim > 0 && batch >= 0, NRC_E_VALUE, "dim must be positive, batch >= 0");
     if (batch == 0) return NRC_OK;
-    mf_pointwise_grad_kernel<<<grad_grid(batch), 256, 0, as_stream(stream)>>>(
-        user_table, item_table, dim, users, items, labels, batch, loss_kind, reg, grad_user,
-        grad_item, touched_user, touched_item, stamp, loss);
+    mf_grad_kernel<false><<<grad_grid(batch), 256, 0, as_stream(stream)>>>(
+        user_table, item_table, dim, users, items, reinterpret_cast<const int32_t*>(labels), batch, loss_kind, reg,
+        grad_user, grad_item, touched_user, touched_item, stamp, loss);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
 }
@@ -927,12 +611,6 @@ extern "C" int nrc_mf_hot_apply(float* hot, float* hot_delta, int64_t n_floats, 
 // BPR with LAZY Adam straight from the train CSR (single GPU): the explicitly-named lazy variant of
 // nrc_mf_bpr_sgd_epoch for tables where TF's dense Adam pass is out of reach.  lr_t = Adam's
 // lr * sqrt(1 - b2^t) / (1 - b1^t) of this step (one value per call = per batch).
-extern "C" int nrc_mf_sgd_set_pipelined(int32_t on) {
-    const int before = sgd_pipe_enabled();
-    g_sgd_pipe = on ? 1 : 0;
-    return before;
-}
-
 extern "C" int nrc_mf_bpr_lazy_adam_epoch(float* user_table, float* user_m, float* user_v, float* item_table, float* item_m,
                                           float* item_v, int32_t dim, const int64_t* train_indptr,
                                           const int32_t* train_indices, const int32_t* pos_users, const int32_t* pos_items,

@@ -480,12 +480,6 @@ def opt_apply_multi(opt, variables, stamp, hyper):
     _count()
 
 
-def mf_sgd_set_pipelined(on):
-    """Kernel behind mf_bpr_sgd_epoch for dim 64 / 128: False (default) the register form, True the bulk-copy
-    pipeline (nrc_mf_sgd_set_pipelined).  Returns the previous setting."""
-    return bool(_lib.load().nrc_mf_sgd_set_pipelined(1 if on else 0))
-
-
 def spmm_set_exact(on):
     """True: sequential, separately rounded accumulation (bit-identical to scipy / TF's CPU kernel);
     False (default): the fast order (nrc_spmm_set_exact)."""

@@ -169,17 +169,8 @@ def test_fused_epoch_equals_the_two_kernel_epoch(ml100k):
     assert np.abs(a["V"].cpu().numpy() - b["V"].cpu().numpy()).max() < 2e-6
 
 
-@pytest.fixture(params=["pipelined", "register"])
-def sgd_kernel(request):
-    """Both kernels behind nrc_mf_bpr_sgd_epoch: the register form (default) and the bulk-copy pipeline."""
-    from neurec_b200 import ops
-    before = ops.mf_sgd_set_pipelined(request.param == "pipelined")
-    yield request.param
-    ops.mf_sgd_set_pipelined(before)
-
-
 @pytest.mark.parametrize("dim", [128, 64, 32])
-def test_csr_fed_sgd_kernel_equals_build_then_step(dim, sgd_kernel):
+def test_csr_fed_sgd_kernel_equals_build_then_step(dim):
     """nrc_mf_bpr_sgd_epoch (sampler + shuffle + in-place BPR/SGD in one kernel, BASELINE config 5)
     against (a) nrc_epoch_build + nrc_mf_bpr_sgd_fused on the same positions and (b) the numpy
     restatement, on an epoch without repeated rows (where the in-place step is order-free)."""
@@ -228,7 +219,7 @@ def test_csr_fed_sgd_kernel_equals_build_then_step(dim, sgd_kernel):
         ops.mf_bpr_sgd_epoch(dU, peer.single(dV), *a, 10, n, lr, reg, loss)
 
 
-def test_csr_fed_sgd_kernel_with_repeated_rows_sums_every_contribution(sgd_kernel):
+def test_csr_fed_sgd_kernel_with_repeated_rows_sums_every_contribution():
     """Hot rows (Zipf items, few users): in-place REDs must not lose updates -- with lr so small that
     reads of already-updated rows change the gradient only in second order, the result must match
     the sum of all per-triplet updates computed on the pre-step tables."""
@@ -253,7 +244,7 @@ def test_csr_fed_sgd_kernel_with_repeated_rows_sums_every_contribution(sgd_kerne
 
 
 @pytest.mark.parametrize("dim", [128, 32])
-def test_replicated_head_gives_the_same_tables(dim, sgd_kernel):
+def test_replicated_head_gives_the_same_tables(dim):
     """ShardSet.enable_hot: rows [0, n_hot) are read from the replica and their deltas accumulated next to it;
     after sync_hot + writeback_hot a duplicate-free epoch leaves bit-identical tables (row + (0 + delta) = row +
     delta), and with repeated rows every contribution is summed (first-order check)."""
@@ -302,9 +293,9 @@ def test_replicated_head_gives_the_same_tables(dim, sgd_kernel):
 
 
 @pytest.mark.parametrize("dim", [128, 64])
-def test_csr_fed_sgd_kernel_many_rounds_per_ring_slot(dim, sgd_kernel):
-    """~60 k triplets in one launch: every ring slot of the pipelined kernel is reused several times (one CTA per SM x
-    128 slots per round), with a ragged last round; same first-order check as above plus the loss."""
+def test_csr_fed_sgd_kernel_large_launch_with_uneven_cta_shares(dim):
+    """~60 k triplets in one launch, not a multiple of the grid size, so the persistent grid's CTAs take shares of
+    unequal length: loss and both tables against the sum of the per-triplet gradients."""
     from neurec_b200 import ops
     from neurec_b200.util import peer
     nu, ni = 3000, 20000
