@@ -220,6 +220,19 @@ int nrc_eval_tc_debug_candidates(int32_t pass, const float* user_table, const fl
                                  int32_t* seg_items, void* stream);
 int nrc_eval_tc_last_fallbacks(int32_t* replayed, int32_t* full_replays);
 
+/* Test hook of the NCF family (it reports and changes nothing; every route is chosen by the shape).
+ * nrc_ncf_last_routes: the code paths of the most recent nrc_ncf_grad / nrc_ncf_train_epoch /
+ *   nrc_ncf_epoch_fused / nrc_ncf_scores launch, HOST bookkeeping written when the call launches (a call
+ *   that returns before launching leaves it as it was).  out i32[7]; -1 = not decided by that call:
+ *   [0] per-batch sample kernel: 1 the default-tower kernel (layers [64,32,16]), 0 the generic one;
+ *   [1] batch slices of the per-batch weight-gradient kernel (16 from 64 samples, else 1; 0 without layers);
+ *   [2] epoch kernel dense gradient: 1 4x4 blocks (every width a multiple of 4), 0 lane quartets;
+ *   [3] epoch kernel embedding tables: 1 float4 (widths multiples of 4, 16-byte aligned), 0 scalar;
+ *   [4], [5] epoch kernel: bit l set when layer l takes the split forward / split backward form;
+ *   [6] scores: 1 the tile kernel (layers [64,32,16], mf_dim <= 64), 0 the warp-per-pair kernel.
+ *   nrc_ncf_train_epoch reports its last step. */
+int nrc_ncf_last_routes(int32_t* out);
+
 /* MF.predict(user_ids, None), model/general_recommender/MF.py:120-122 (np.matmul(U[users], V.T))
  * and LightGCN.predict, LightGCN.py:187-189, materialised: scores f32 [num_rows, num_items]
  * with the same fp32 FMA chain over k the fused evaluator uses. */

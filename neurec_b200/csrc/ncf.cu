@@ -32,6 +32,12 @@
 
 namespace nrc {
 
+int32_t g_ncf_routes[kNcfRoutes] = {-1, -1, -1, -1, -1, -1, -1};
+
+void ncf_routes_reset() {
+    for (int r = 0; r < kNcfRoutes; ++r) g_ncf_routes[r] = -1;
+}
+
 int ncf_make(NcfDev& S, const nrc_ncf_shape* sh) {
     NRC_REQUIRE(sh != nullptr, NRC_E_VALUE, "shape is NULL");
     NRC_REQUIRE(sh->n_layers >= 0 && sh->n_layers <= kNcfMaxLayers, NRC_E_LIMIT,
@@ -623,6 +629,10 @@ static int ncf_launch_grad(const nrc_ncf_shape* shape, const NcfPtrs& P, const i
     NRC_REQUIRE(smem <= 48 * 1024, NRC_E_LIMIT, "NCF tower too wide: %zu B of shared memory", smem);
     const bool fast = S.n_layers == 3 && S.in_dim[0] == 64 && S.out_dim[0] == 64 &&
                       S.out_dim[1] == 32 && S.out_dim[2] == 16;
+    const int slices = (batch >= 64) ? kWgradSlices : 1;
+    ncf_routes_reset();
+    g_ncf_routes[kRouteSampleFast] = fast ? 1 : 0;
+    g_ncf_routes[kRouteWgradSlices] = S.n_layers > 0 ? slices : 0;
     if (fast)
         ncf_sample_fast_kernel<64, 64, 32, 16><<<(unsigned)batch, kNcfThreads, 0, st>>>(
             S, P, users, items, third, batch, pairwise, loss_kind, reg_mf, reg_mlp, stamp, g_scratch, loss);
@@ -632,7 +642,6 @@ static int ncf_launch_grad(const nrc_ncf_shape* shape, const NcfPtrs& P, const i
                                                                       stamp, g_scratch, loss);
     NRC_CUDA_CHECK(cudaGetLastError());
     if (S.n_layers > 0) {
-        const int slices = (batch >= 64) ? kWgradSlices : 1;
         int max_in = 0, max_out = 0;
         for (int l = 0; l < S.n_layers; ++l) {
             max_in = S.in_dim[l] > max_in ? S.in_dim[l] : max_in;
@@ -653,6 +662,13 @@ extern "C" int nrc_ncf_dense_size(const nrc_ncf_shape* shape) {
     NcfDev S;
     if (ncf_make(S, shape)) return NRC_E_VALUE;
     return S.tower_size * S.n_towers;
+}
+
+// Host bookkeeping of the code paths the most recent NCF call launched (see the header); no device work.
+extern "C" int nrc_ncf_last_routes(int32_t* out) {
+    NRC_REQUIRE(out != nullptr, NRC_E_VALUE, "NULL output");
+    for (int r = 0; r < kNcfRoutes; ++r) out[r] = g_ncf_routes[r];
+    return NRC_OK;
 }
 
 extern "C" int nrc_ncf_grad(const nrc_ncf_shape* shape, const float* mf_user, const float* mf_item,
@@ -702,6 +718,8 @@ extern "C" int nrc_ncf_scores(const nrc_ncf_shape* shape, const float* mf_user, 
             NRC_CUDA_CHECK(cudaFuncSetAttribute(ncf_scores_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
             fattr = true;
         }
+        ncf_routes_reset();
+        g_ncf_routes[kRouteScoresTile] = 1;
         const int64_t units = (int64_t)((n_users + kTileUsers - 1) / kTileUsers) * ((num_items + kTileItems - 1) / kTileItems);
         int64_t grid = (int64_t)sm_count();
         if (grid > units) grid = units;
@@ -728,6 +746,8 @@ extern "C" int nrc_ncf_scores(const nrc_ncf_shape* shape, const float* mf_user, 
         NRC_CUDA_CHECK(cudaFuncSetAttribute(ncf_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         attr_done = true;
     }
+    ncf_routes_reset();
+    g_ncf_routes[kRouteScoresTile] = 0;
     const int64_t total = (int64_t)n_users * num_items;
     int64_t blocks = (total + kNcfWarps - 1) / kNcfWarps;
     const int64_t cap = (int64_t)sm_count() * 4;

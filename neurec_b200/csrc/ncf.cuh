@@ -27,4 +27,19 @@ struct NcfPtrs {
 
 int ncf_make(NcfDev& S, const nrc_ncf_shape* sh);
 
+// Layer forms of the epoch kernel's tower (ncf_epoch.cu fwd_layer / bwd_layer), one copy for the kernel and
+// for the route hook.  Forward split: the k-range of a layer is divided over kNcfThreads / out thread groups.
+// Backward split: kNcfThreads / in threads (at most a warp) share each input row k.  Macros, not functions:
+// with the same condition behind a __host__ __device__ function nvcc 12.9 compiled a different, larger
+// ncf_epoch_kernel; the macros leave its SASS as it was with the conditions written inline.
+#define NCF_FWD_SPLIT(in, out) ((out) <= kNcfThreads && kNcfThreads % (out) == 0 && (in) % (kNcfThreads / (out)) == 0)
+#define NCF_BWD_SPLIT(in, out) \
+    ((in) <= kNcfThreads && kNcfThreads % (in) == 0 && (kNcfThreads / (in)) <= 32 && (out) % (kNcfThreads / (in)) == 0)
+
+// Routes of the most recent NCF launch (nrc_ncf_last_routes); -1 = not decided by that call.
+enum NcfRoute { kRouteSampleFast, kRouteWgradSlices, kRouteEpochDwBlocked, kRouteEpochTablesVec4, kRouteFwdSplit,
+                kRouteBwdSplit, kRouteScoresTile, kNcfRoutes };
+extern int32_t g_ncf_routes[kNcfRoutes];
+void ncf_routes_reset();
+
 }  // namespace nrc

@@ -75,7 +75,7 @@ __device__ __forceinline__ float group_sum(float v, float* red, int tid, int grp
 // a_out = relu(a_in . W + b); W in shared memory exactly as in global memory (row stride out)
 __device__ __forceinline__ void fwd_layer(const float* __restrict__ W, const float* __restrict__ B, int in, int out,
                                           const float* a_in, float* a_out, float* part, int tid, int grp) {
-    if (out <= kNcfThreads && kNcfThreads % out == 0 && in % (kNcfThreads / out) == 0) {
+    if (NCF_FWD_SPLIT(in, out)) {
         const int G = kNcfThreads / out, kpg = in / G, j = tid % out, g = tid / out;
         float acc = 0.0f;
 #pragma unroll 8
@@ -102,7 +102,7 @@ __device__ __forceinline__ void fwd_layer(const float* __restrict__ W, const flo
 // banks of the unpadded row-major W.
 __device__ __forceinline__ void bwd_layer(const float* __restrict__ W, int in, int out, const float* d_out,
                                           const float* a_in, float* d_in, bool mask, int tid, int grp) {
-    if (in <= kNcfThreads && kNcfThreads % in == 0 && (kNcfThreads / in) <= 32 && out % (kNcfThreads / in) == 0) {
+    if (NCF_BWD_SPLIT(in, out)) {
         const int tpr = kNcfThreads / in, jpt = out / tpr, k = tid / tpr, jq = tid % tpr;
         float s = 0.0f;
         int jj = k % jpt;
@@ -537,6 +537,14 @@ extern "C" int nrc_ncf_epoch_fused(const nrc_ncf_shape* shape, float* mf_user, f
     int per_sm = 0;
     NRC_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ncf_epoch_kernel, kEpThreads, smem));
     NRC_REQUIRE(per_sm >= 1, NRC_E_CUDA, "the persistent NCF epoch kernel does not fit an SM");
+    ncf_routes_reset();
+    g_ncf_routes[kRouteEpochDwBlocked] = Q.wblocked;
+    g_ncf_routes[kRouteEpochTablesVec4] = Q.tables_vec4;
+    g_ncf_routes[kRouteFwdSplit] = g_ncf_routes[kRouteBwdSplit] = 0;
+    for (int l = 0; l < S.n_layers; ++l) {
+        if (NCF_FWD_SPLIT(S.in_dim[l], S.out_dim[l])) g_ncf_routes[kRouteFwdSplit] |= 1 << l;
+        if (NCF_BWD_SPLIT(S.in_dim[l], S.out_dim[l])) g_ncf_routes[kRouteBwdSplit] |= 1 << l;
+    }
     void* args[] = {&Q};
     NRC_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)ncf_epoch_kernel, dim3(sm_count()), dim3(kEpThreads), args, smem, st));
     return NRC_OK;

@@ -567,6 +567,18 @@ class NcfShape(ctypes.Structure):
         return n
 
 
+NCF_ROUTES = ("sample_fast", "wgrad_slices", "epoch_dw_blocked", "epoch_tables_vec4", "fwd_split", "bwd_split",
+              "scores_tile")
+
+
+def ncf_last_routes():
+    """Code paths of the most recent NCF launch (nrc_ncf_last_routes) as {name: value}; -1 = not decided by it.
+    fwd_split / bwd_split are bitmasks over the epoch kernel's layers."""
+    out = (ctypes.c_int32 * len(NCF_ROUTES))()
+    check(_lib.load().nrc_ncf_last_routes(out))
+    return dict(zip(NCF_ROUTES, out))
+
+
 def ncf_grad(shape, P, users, items, third, pairwise, loss, reg_mf, reg_mlp, G, tU, tI, stamp,
              loss_out):
     """P / G: dicts with keys mf_user, mf_item, mlp_user, mlp_item, dense (tensors or None)."""
