@@ -786,6 +786,23 @@ int nrc_spectralcf_grad(int32_t num_users, int32_t num_items, int32_t dim, int32
                         int32_t loss_kind, float reg, float* all_emb, float* grad_all, int32_t* touched,
                         float* grad_e0, float* grad_filters, float* work, float* loss, void* stream);
 
+/* WRMF, model/general_recommender/WRMF.py:51-61,69-85: one ALS half-step, every row of a CSR solved in one call.
+ * For row r with CSR entries J(r) over the fixed table Y (fixed f32 [num_fixed, dim]):
+ *   x_r = (Y^T Y + alpha * sum_{j in J(r)} y_j y_j^T + reg * I)^-1 (1 + alpha) sum_{j in J(r)} y_j
+ * written to out f32 [num_rows, dim] (out must not alias fixed).  The user half passes the user-major CSR and the
+ * item table, the item half the item-major CSR and the user table just written; an empty row gets x = 0.  Y^T Y is
+ * summed over fixed slices of num_fixed, then in a fixed order, and made exactly symmetric; each row is factored by
+ * Cholesky with one fixed summation order, so the result is bit-reproducible and independent of which other rows
+ * are in the call.  row_order i32 [num_rows] (a permutation: the order rows are scheduled in, heaviest first), or
+ * NULL for 0 .. num_rows - 1.  work f32 [nrc_wrmf_work_floats(max(num_fixed), dim)].  *not_spd (device i32) is set
+ * to the number of rows whose matrix had a pivot that was not positive and finite; those rows are left unchanged
+ * (impossible with reg > 0).  NRC_E_LIMIT when dim is outside [1, 128]; NRC_E_VALUE when alpha or reg is negative
+ * or not finite (the reference's LU solve would still return a value there).  A rejected call writes nothing. */
+int64_t nrc_wrmf_work_floats(int32_t num_rows_max, int32_t dim);
+int nrc_wrmf_half_step(const float* fixed, int32_t num_fixed, const int64_t* indptr, const int32_t* indices,
+                       const int32_t* row_order, int32_t num_rows, int32_t dim, float alpha, float reg, float* out,
+                       float* work, int32_t* not_spd, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

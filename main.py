@@ -29,7 +29,7 @@ def resolve_model(recommender):
         if importlib.util.find_spec(name) is not None:
             return getattr(importlib.import_module(name), recommender)
     raise ImportError("recommender '%s' is outside the accelerated hot path "
-                      "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, SBPR)" % recommender)
+                      "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, WRMF, SBPR)" % recommender)
 
 
 if __name__ == "__main__":

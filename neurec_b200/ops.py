@@ -855,6 +855,38 @@ def spectralcf_grad(num_users, a_hat, a_hat_t, e0, filters, activation, users, p
     _count(3 + 6 * K)
 
 
+def wrmf_work(num_rows_max, dim, device="cuda"):
+    n = int(_lib.load().nrc_wrmf_work_floats(int(num_rows_max), int(dim)))
+    return torch.empty((max(n, 1),), dtype=torch.float32, device=device)
+
+
+def wrmf_half_step(fixed, indptr, indices, out, alpha, reg, row_order=None, work=None, not_spd=None):
+    """One WRMF half-step (WRMF.py:51-61): every row of the CSR (indptr, indices) over the fixed table is solved
+    in one call and written to out f32 [len(indptr) - 1, dim].  NrcError naming the count when some rows' matrices
+    are not positive definite (those rows are left unchanged)."""
+    _req(fixed, torch.float32, "fixed"); _req(out, torch.float32, "out")
+    _req(indptr, torch.int64, "indptr"); _req(indices, torch.int32, "indices")
+    if row_order is not None:
+        _req(row_order, torch.int32, "row_order")
+    num_fixed, dim = fixed.shape
+    num_rows = indptr.numel() - 1
+    if out.shape != (num_rows, dim):
+        raise ValueError("out must be [%d, %d], got %s" % (num_rows, dim, tuple(out.shape)))
+    work = wrmf_work(num_fixed, dim, fixed.device) if work is None else _req(work, torch.float32, "work")
+    if work.numel() < _lib.load().nrc_wrmf_work_floats(num_fixed, dim):
+        raise ValueError("work holds %d floats, the call needs nrc_wrmf_work_floats(%d, %d)" % (work.numel(), num_fixed, dim))
+    if not_spd is None:
+        not_spd = torch.empty((1,), dtype=torch.int32, device=fixed.device)
+    check(_lib.load().nrc_wrmf_half_step(_p(fixed), num_fixed, _p(indptr), _p(indices), _p(row_order), num_rows, dim,
+                                         float(alpha), float(reg), _p(out), _p(work), _p(not_spd), _stream()))
+    _count(3)
+    bad = int(not_spd.item())
+    if bad:
+        raise _lib.NrcError("WRMF: %d of %d rows have a matrix that is not positive definite (reg_mf = %g); "
+                            "they were left unchanged" % (bad, num_rows, reg))
+    return out
+
+
 def split_interactions(users, keys, num_users, mode="ratio", ratio=0.8, seed=0):
     """Per-user train / test split of an interaction list on the device (data/utils.py:59-106): int32 [n] of 1 (train)
     / 0 (test).  keys: int64 CUDA tensor of interaction times (by_time=True) or None (by_time=False)."""
