@@ -187,10 +187,10 @@ static int launch_bpr_sgd(const RowShards& SU, const RowShards& SV, int dim, con
 // The same single-pass step fed straight from the train CSR: positions [first, first + count) of
 // the shuffled epoch (epoch.cuh) are sampled INSIDE the kernel -- no id arrays in HBM, no sampler
 // or shuffle pass in front (data/sampler.py:71-90,189-206 + util/data_iterator.py:59 fused in).
-// A persistent grid (as many 256-thread CTAs as fit, 3 per SM) splits [first, first + count) evenly;
-// a CTA takes its share 256 consecutive positions at a time:
+// A persistent grid (one 768-thread CTA per SM) splits [first, first + count) evenly;
+// a CTA takes its share 768 consecutive positions at a time:
 //   phase a  one THREAD per triplet: bijection -> (user, positive) -> Philox rejection draw against
-//            the user's sorted row; ~10 dependent loads, 256 chains in flight per CTA;
+//            the user's sorted row; ~10 dependent loads, 768 chains in flight per CTA;
 //   phase b  one WARP per triplet, two triplets in flight per warp: row gathers (float4 per lane),
 //            shuffle-reduced dots, in-place vector RED.ADD (the hottest head rows: shared memory, below).
 // On one H100 vector REDs were as fast as one bulk reduce-add per row (cp.reduce.async.bulk) and need
@@ -238,11 +238,16 @@ __device__ __forceinline__ void update_item(const RowShards& V, int32_t id, int 
     }
 }
 
+// One CTA of 768 threads per SM: one copy of the tier per SM leaves the rest of the SM's shared memory to L1 and flushes
+// one set of tier deltas per SM.  On one H100 it measured 3 % faster than three CTAs of 256 threads (three tier copies)
+// and than two of 384 or 512 (profiles/r4_sgd_breakdown_n1.json).
+constexpr int kStreamThreads = 768;
+
 template <int VEC, bool SHARDED>
-__global__ void __launch_bounds__(256, 3)
+__global__ void __launch_bounds__(kStreamThreads, 1)
 mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const EpochSpec E, int64_t first,
                          int64_t count, float lr, float reg, float* __restrict__ loss) {
-    constexpr int D = 32 * VEC, CH = 256, T = kSgdTierRows<VEC>;
+    constexpr int D = 32 * VEC, CH = kStreamThreads, T = kSgdTierRows<VEC>;
     constexpr int TPW = 2;                     // triplets in flight per warp (3 and 4 measured slower)
     __shared__ int32_t s_u[CH], s_i[CH], s_j[CH];
     extern __shared__ __align__(16) float s_tier[];
@@ -254,7 +259,7 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
         reinterpret_cast<float4*>(s_val)[e] = reinterpret_cast<const float4*>(V.hot)[e];
         reinterpret_cast<float4*>(s_dlt)[e] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    // an even share of [0, count) per CTA of the persistent grid, sampled 256 positions at a time
+    // an even share of [0, count) per CTA of the persistent grid, sampled kStreamThreads positions at a time
     const int64_t lo = count * blockIdx.x / gridDim.x, hi = count * (blockIdx.x + 1) / gridDim.x;
     float loss_acc = 0.0f;
     for (int64_t c0 = lo; c0 < hi; c0 += CH) {
@@ -266,7 +271,7 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
         }
         __syncthreads();
         // TPW triplets per warp in flight: all 3 * TPW row loads are issued before the first is used
-        for (int t0 = warp * TPW; t0 < n; t0 += 8 * TPW) {
+        for (int t0 = warp * TPW; t0 < n; t0 += (kStreamThreads / 32) * TPW) {
             float a[TPW][VEC], b[TPW][VEC], c[TPW][VEC];
 #pragma unroll
             for (int k = 0; k < TPW; ++k) {
@@ -331,13 +336,13 @@ static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E
         NRC_CUDA_CHECK(cudaFuncSetAttribute(mf_bpr_sgd_stream_kernel<VEC, SH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)smem));
         int per_sm = 0;
-        NRC_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mf_bpr_sgd_stream_kernel<VEC, SH>, 256, smem));
+        NRC_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mf_bpr_sgd_stream_kernel<VEC, SH>, kStreamThreads, smem));
         NRC_REQUIRE(per_sm > 0, NRC_E_CUDA, "mf_bpr_sgd_stream_kernel does not fit on an SM");
         grid_cap = (int64_t)per_sm * sm_count();
     }
-    int64_t blocks = (count + 255) / 256;
+    int64_t blocks = (count + kStreamThreads - 1) / kStreamThreads;
     if (blocks > grid_cap) blocks = grid_cap;
-    mf_bpr_sgd_stream_kernel<VEC, SH><<<(unsigned)blocks, 256, smem, st>>>(U_local, SV, E, first, count, lr, reg, loss);
+    mf_bpr_sgd_stream_kernel<VEC, SH><<<(unsigned)blocks, kStreamThreads, smem, st>>>(U_local, SV, E, first, count, lr, reg, loss);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
 }

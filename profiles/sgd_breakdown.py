@@ -15,7 +15,9 @@ into OUT.json under NAME, next to the card's name and power limit read in the sa
   prebuilt_ids   ids of the same positions built by ops.epoch_build beforehand (untimed), then ops.mf_bpr_sgd_fused
                  timed, against the CSR-fed kernel on the same tables in the same process (both without a head)
   probe          profiles/row_update_probe.cu: read / read + store / read + RED.v4 / read + bulk reduce-add of 3 x 2^20
-                 rows of a 12.5 M x 128 table; row ids uniform, Zipf, and the step's mix of the two
+                 rows of a 12.5 M x 128 table; row ids uniform, Zipf, and the step's mix of the two; and read + store
+                 where no other id of the launch names the row, RED.v4 elsewhere (store_if_single), against RED.v4
+                 everywhere, on the rows one step updates in place outside the head (step_cold)
 """
 import argparse
 import json
