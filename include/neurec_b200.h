@@ -418,7 +418,11 @@ int nrc_mf_bpr_sgd_sharded(float* const* user_shards, float* const* item_shards,
  * owner); item ids are global, item_shards[r] (host array of `world` device pointers) is the row
  * block of rank r: own memory for r == self_rank, peer mappings otherwise (nrc_shard_alloc /
  * nrc_ipc_open), read and RED-updated over NVLink by the same kernel.  world = 1: item_shards[0]
- * is the whole table.  *loss += sum of the triplets' losses. */
+ * is the whole table.  *loss += sum of the triplets' losses.
+ * When pos_items == train_indices (the same pointer), pos_users MUST be the row expansion of
+ * train_indptr (pos_users[q] = u for q in [train_indptr[u], train_indptr[u+1]), as nrc_csr_row_ids
+ * writes it): the kernel then finds the user rows that only one triplet of the call touches from the
+ * CSR and the shuffle alone, and writes those with plain stores instead of atomics. */
 int nrc_mf_bpr_sgd_epoch(float* user_table, float* const* item_shards, int32_t world,
                          int32_t self_rank, int64_t items_per_shard, int32_t dim,
                          const int64_t* train_indptr, const int32_t* train_indices,

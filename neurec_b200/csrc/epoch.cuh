@@ -62,6 +62,29 @@ __host__ __device__ __forceinline__ int64_t feistel_perm(const Feistel& F, int64
     return (int64_t)x;
 }
 
+// The network run backwards: round r maps (L, R) back to (R ^ (F(L, k_r) & mask(|R|)), L).  After an even number of
+// rounds the halves have their initial widths again, so the output splits as the input did.
+static_assert(kFeistelRounds % 2 == 0, "feistel_once_inv assumes the halves end at their initial widths");
+__host__ __device__ __forceinline__ uint64_t feistel_once_inv(const Feistel& F, uint64_t x) {
+    int bl = F.bits_l, br = F.bits_r;
+    uint32_t L = (uint32_t)(x >> br), R = (uint32_t)(x & ((1ull << br) - 1ull));
+#pragma unroll
+    for (int r = kFeistelRounds - 1; r >= 0; --r) {
+        const uint32_t pl = R ^ (feistel_mix(L, F.key[r]) & (uint32_t)((1ull << br) - 1ull));
+        R = L; L = pl;
+        const int t = bl; bl = br; br = t;
+    }
+    return ((uint64_t)L << br) | R;
+}
+
+// perm^-1: the shuffled position at which unshuffled index q is visited (walks the cycle backwards)
+__host__ __device__ __forceinline__ int64_t feistel_perm_inv(const Feistel& F, int64_t q) {
+    if (!F.shuffle) return q;
+    uint64_t x = (uint64_t)q;
+    do { x = feistel_once_inv(F, x); } while (x >= F.n);
+    return (int64_t)x;
+}
+
 // What an epoch is made of (all device pointers).
 struct EpochSpec {
     const int64_t* tptr;    // train CSR row pointers [num_users + 1]

@@ -190,9 +190,12 @@ static int launch_bpr_sgd(const RowShards& SU, const RowShards& SV, int dim, con
 // A persistent grid (one 768-thread CTA per SM) splits [first, first + count) evenly;
 // a CTA takes its share 768 consecutive positions at a time:
 //   phase a  one THREAD per triplet: bijection -> (user, positive) -> Philox rejection draw against
-//            the user's sorted row; ~10 dependent loads, 768 chains in flight per CTA;
+//            the user's sorted row; ~10 dependent loads, 768 chains in flight per CTA.  When the
+//            positives are the CSR itself, also whether any other position of the launch visits one
+//            of the user's positives (perm^-1 of each: arithmetic only, no loads);
 //   phase b  one WARP per triplet, two triplets in flight per warp: row gathers (float4 per lane),
-//            shuffle-reduced dots, in-place vector RED.ADD (the hottest head rows: shared memory, below).
+//            shuffle-reduced dots, in-place vector RED.ADD (the hottest head rows: shared memory, below);
+//            a user row no other triplet touches gets a plain store of value + delta instead.
 // On one H100 vector REDs were as fast as one bulk reduce-add per row (cp.reduce.async.bulk) and need
 // no staging buffer (profiles/r3_sgd_breakdown_n1.json).
 // User rows are always local (the train CSR is sharded by user owner, SURVEY 8e); item rows may
@@ -238,6 +241,40 @@ __device__ __forceinline__ void update_item(const RowShards& V, int32_t id, int 
     }
 }
 
+// The add a float RED performs (round to nearest, subnormals flushed): never contracted with the multiply that made d
+__device__ __forceinline__ float add_as_red(float x, float d) {
+    float r;
+    asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(d));
+    return r;
+}
+
+// Positives of a user at most this long are checked for other visits in the launch (one inverse bijection each);
+// longer rows always take the RED.
+constexpr int64_t kOnceMaxRow = 32;
+constexpr int32_t kUserOnce = INT32_MIN;   // bit 31 of s_u: the user row is touched by this triplet alone
+
+// Pairwise sample at shuffled position p (epoch_sample with k = 0, the same bits).  With `user_once`, u carries
+// kUserOnce when no other position of [first, first + count) visits one of the user's positives: the positives are CSR
+// positions [beg, end) (pos_users is the row expansion of tptr), and the position visiting q is perm^-1(q).
+__device__ __forceinline__ void stream_sample(const EpochSpec& E, int64_t p, int64_t first, int64_t count, bool user_once,
+                                              int32_t& u, int32_t& item, int32_t& third) {
+    const int64_t idx = feistel_perm(E.perm, p);
+    u = __ldg(E.users + idx);
+    item = __ldg(E.pos + idx);
+    const int64_t beg = __ldg(E.tptr + u), end = __ldg(E.tptr + u + 1);
+    third = philox_draw_excluding((uint64_t)(idx * E.neg_num), E.seed, E.stream_id, E.num_items, E.tidx + beg, end - beg);
+    if (user_once && end - beg <= kOnceMaxRow) {
+        bool alone = true;
+#pragma unroll 1
+        for (int64_t q = beg; q < end; ++q) {
+            if (q == idx) continue;
+            const int64_t r = feistel_perm_inv(E.perm, q);
+            alone &= (uint64_t)(r - first) >= (uint64_t)count;
+        }
+        if (alone) u |= kUserOnce;
+    }
+}
+
 // One CTA of 768 threads per SM: one copy of the tier per SM leaves the rest of the SM's shared memory to L1 and flushes
 // one set of tier deltas per SM.  On one H100 it measured 3 % faster than three CTAs of 256 threads (three tier copies)
 // and than two of 384 or 512 (profiles/r4_sgd_breakdown_n1.json).
@@ -246,10 +283,10 @@ constexpr int kStreamThreads = 768;
 template <int VEC, bool SHARDED>
 __global__ void __launch_bounds__(kStreamThreads, 1)
 mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const EpochSpec E, int64_t first,
-                         int64_t count, float lr, float reg, float* __restrict__ loss) {
+                         int64_t count, int user_once, float lr, float reg, float* __restrict__ loss) {
     constexpr int D = 32 * VEC, CH = kStreamThreads, T = kSgdTierRows<VEC>;
     constexpr int TPW = 2;                     // triplets in flight per warp (3 and 4 measured slower)
-    __shared__ int32_t s_u[CH], s_i[CH], s_j[CH];
+    __shared__ int32_t s_u[CH], s_i[CH], s_j[CH];   // s_u: user id | kUserOnce (stream_sample)
     extern __shared__ __align__(16) float s_tier[];
     float* const s_val = s_tier;               // [T][D] pre-step values of head rows [0, nt)
     float* const s_dlt = s_tier + T * D;       // [T][D] this CTA's summed deltas of those rows
@@ -266,7 +303,7 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
         const int n = (hi - c0 < CH) ? (int)(hi - c0) : CH;
         if ((int)threadIdx.x < n) {
             int32_t u, i, j;
-            epoch_sample(E, first + c0 + threadIdx.x, 0, u, i, j);
+            stream_sample(E, first + c0 + threadIdx.x, first, count, user_once != 0, u, i, j);
             s_u[threadIdx.x] = u; s_i[threadIdx.x] = i; s_j[threadIdx.x] = j;
         }
         __syncthreads();
@@ -276,7 +313,7 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
 #pragma unroll
             for (int k = 0; k < TPW; ++k) {
                 const int t = (t0 + k < n) ? t0 + k : t0;
-                ld_vec<VEC>(U_local + (size_t)s_u[t] * D + lane * VEC, a[k]);
+                ld_vec<VEC>(U_local + (size_t)(s_u[t] & ~kUserOnce) * D + lane * VEC, a[k]);
                 load_item<VEC, SHARDED>(V, s_i[t], nt, s_val, lane, b[k]);
                 load_item<VEC, SHARDED>(V, s_j[t], nt, s_val, lane, c[k]);
             }
@@ -307,7 +344,15 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
                     dvi[q] = -lr * (g * a[k][q] + reg * b[k][q]);
                     dvj[q] = -lr * (-g * a[k][q] + reg * c[k][q]);
                 }
-                red_row<VEC>(U_local + (size_t)s_u[t] * D + lane * VEC, du, false);
+                const int32_t su = s_u[t];
+                float* const pu = U_local + (size_t)(su & ~kUserOnce) * D + lane * VEC;
+                if (su & kUserOnce) {   // no other triplet of the launch reads or writes the row: a + du is what RED leaves
+#pragma unroll
+                    for (int q = 0; q < VEC; ++q) du[q] = add_as_red(a[k][q], du[q]);
+                    st_vec<VEC>(pu, du);
+                } else {
+                    red_row<VEC>(pu, du, false);
+                }
                 update_item<VEC, SHARDED>(V, s_i[t], nt, s_dlt, lane, dvi);
                 update_item<VEC, SHARDED>(V, s_j[t], nt, s_dlt, lane, dvj);
             }
@@ -328,8 +373,8 @@ mf_bpr_sgd_stream_kernel(float* __restrict__ U_local, const RowShards V, const E
 }
 
 template <int VEC, bool SH>
-static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E, int64_t first, int64_t count, float lr,
-                         float reg, float* loss, cudaStream_t st) {
+static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E, int64_t first, int64_t count,
+                         int user_once, float lr, float reg, float* loss, cudaStream_t st) {
     constexpr size_t smem = kSgdTierBytes<VEC>;
     static int64_t grid_cap = 0;     // the persistent grid: as many CTAs as fit on the device at once
     if (!grid_cap) {
@@ -342,7 +387,8 @@ static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E
     }
     int64_t blocks = (count + kStreamThreads - 1) / kStreamThreads;
     if (blocks > grid_cap) blocks = grid_cap;
-    mf_bpr_sgd_stream_kernel<VEC, SH><<<(unsigned)blocks, kStreamThreads, smem, st>>>(U_local, SV, E, first, count, lr, reg, loss);
+    mf_bpr_sgd_stream_kernel<VEC, SH><<<(unsigned)blocks, kStreamThreads, smem, st>>>(U_local, SV, E, first, count,
+                                                                                      user_once, lr, reg, loss);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
 }
@@ -350,8 +396,10 @@ static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E
 static int launch_bpr_sgd_stream(float* U_local, const RowShards& SV, int dim, const EpochSpec& E, int64_t first,
                                  int64_t count, float lr, float reg, float* loss, cudaStream_t st) {
     const bool sharded = SV.rows_per_shard != 0;
-#define NRC_STREAM(VEC) (sharded ? launch_stream<VEC, true>(U_local, SV, E, first, count, lr, reg, loss, st) \
-                                 : launch_stream<VEC, false>(U_local, SV, E, first, count, lr, reg, loss, st))
+    // user rows touched once are found from the CSR: only when the positives are the CSR itself
+    const int user_once = E.pos == E.tidx ? 1 : 0;
+#define NRC_STREAM(VEC) (sharded ? launch_stream<VEC, true>(U_local, SV, E, first, count, user_once, lr, reg, loss, st) \
+                                 : launch_stream<VEC, false>(U_local, SV, E, first, count, user_once, lr, reg, loss, st))
     if (dim == 128) return NRC_STREAM(4);
     if (dim == 64) return NRC_STREAM(2);
     return NRC_STREAM(1);
