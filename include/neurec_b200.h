@@ -141,7 +141,12 @@ int nrc_arg_topk_host(const float* scores, int32_t rating_len, int32_t rows_num,
  * The [B, num_items] score matrix is never materialised.
  *   user_table f32 [*, dim], item_table f32 [num_items, dim]
  *   users i32 [num_eval_users]; train/test CSR are indexed by USER ID.
- *   results f32 [num_eval_users, metric_num*top_k]; ranks optional. */
+ *   results f32 [num_eval_users, metric_num*top_k]; ranks optional.
+ * Envelope: the heap-replay kernel keeps 64 user rows, a 64-item tile and 64 heaps in shared
+ * memory, so with D4 = dim rounded up to a multiple of 4 and L = min(2*top_k, num_items) a shape
+ * is accepted when 256 * (2*D4 + 4 + 2*L + 3*top_k) <= 227 * 1024, i.e. 2*D4 + 2*L + 3*top_k <= 904
+ * (dim <= 448; top_k <= 128 at dim 1, 110 at dim 64, 92 at dim 128 when num_items >= 2*top_k).
+ * Other shapes return NRC_E_LIMIT and leave the outputs untouched. */
 int nrc_eval_mf(const float* user_table, const float* item_table, int32_t dim,
                 int32_t num_items, const int32_t* users, int32_t num_eval_users,
                 const int64_t* train_indptr, const int32_t* train_indices,
@@ -156,6 +161,17 @@ int nrc_eval_mf(const float* user_table, const float* item_table, int32_t dim,
 int nrc_eval_force_exact(int32_t on);
 /* How many users of the last nrc_eval_mf / nrc_eval_mf_tc call needed a heap replay (host int32 out). */
 int nrc_eval_last_undecided(int32_t* count_host);
+/* Test hook of the evaluator (it reports and changes nothing; every route is chosen by the shape):
+ * HOST bookkeeping written when a call launches, out i32[3], -1 = no such launch yet.  It is one
+ * record per process, not per thread: with several host threads it shows whichever launched last.
+ *   [0] selection form of the last nrc_eval_mf: 0 heap replay for every user (top_k >= 32 or
+ *       nrc_eval_force_exact), 1 fast pass with 2 users per warp (<= 16 users per SM), 2 fast pass
+ *       on 128-item tiles, 3 fast pass on 64-item tiles (dim too large for the 128-item tile);
+ *       every fast form is followed by the heap replay of the users it could not decide;
+ *   [1] 1 when the last eval_rows_kernel launch (nrc_eval_score_matrix[_host], nrc_arg_topk[_host])
+ *       ran its fast pass, 0 when it replayed the heap for every row;
+ *   [2] that launch's warps per CTA (8, fewer when 2*L + 3*top_k words per warp exceed 12 KB). */
+int nrc_eval_last_routes(int32_t* out);
 
 /* nrc_eval_mf for large catalogues (BASELINE config 4) with the score step on the Hopper tensor
  * cores: bf16 copies of the tables, wgmma (64 users x 128 items x k16 per warpgroup, 64 items at
@@ -255,8 +271,9 @@ int nrc_mask_rows(float* scores, int32_t rating_len, int32_t num_rows, const int
  *                             indexed by ROW in the same id space; masked / missing -> -inf
  *   nrc_eval_merge_candidates per row the K best of C (score, GLOBAL id) candidates in (score desc,
  *                             id asc) order + the metrics of metric.h on them; *tie_count += rows
- *                             with equal scores inside their top K+1 (there the reference's order
- *                             depends on its heap and only the score sequence is guaranteed equal) */
+ *                             with equal scores inside their top K+1, fewer than K+1 candidates or a
+ *                             NaN candidate (there the reference's order depends on its heap and only
+ *                             the score sequence is guaranteed equal); top_k <= 512, C <= 512 */
 int nrc_mf_score_pairs(const float* user_rows, const float* item_table, int32_t dim,
                        const int32_t* items, int32_t num_rows, int32_t C, const int64_t* train_indptr,
                        const int32_t* train_indices, float* out, void* stream);
@@ -267,7 +284,8 @@ int nrc_eval_merge_candidates(const int32_t* cand_ids, const float* cand_scores,
 
 /* np.mean(all_user_result, axis=0) in fp32, evaluator/backend/cpp/uni_evaluator.py:150:
  * out[c] = (sequential fp32 sum over rows of results[:, c]) / num_rows, bit-identical to
- * numpy's axis-0 reduction order. */
+ * numpy's axis-0 reduction order; a single column is contiguous, and there numpy's (and this
+ * call's) sum is pairwise. */
 int nrc_mean_rows(const float* results, int64_t num_rows, int32_t num_cols, float* out,
                   void* stream);
 

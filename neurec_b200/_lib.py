@@ -27,7 +27,11 @@ _CT = {
 
 
 class NrcError(RuntimeError):
-    pass
+    """`rc` is the NRC_E_* code of a failed call (None when the library could not be loaded)."""
+
+    def __init__(self, msg, rc=None):
+        super().__init__(msg)
+        self.rc = rc
 
 
 def declared_functions(header: str = HEADER):
@@ -83,4 +87,4 @@ def check(rc: int) -> None:
         raise TypeError(msg)
     if rc == NRC_E_NOTIMPL:
         raise NotImplementedError(msg)
-    raise NrcError("neurec_b200 error %d: %s" % (rc, msg))
+    raise NrcError("neurec_b200 error %d: %s" % (rc, msg), rc)

@@ -257,8 +257,12 @@ eval_rows_kernel(const float* __restrict__ scores, int N, int rows, int K, int L
                 }
             }
         }
+        // A NaN among the L items that seed the reference's heap changes its ranking (no comparison
+        // with it holds); the fast pass never inserts NaN, so such rows take the heap replay.  A NaN
+        // at i >= L is never admitted by the reference either.  L <= 2K <= 62 here.
+        const bool seed_nan = (lane < L && isnan(r[lane])) || (lane + kWarp < L && isnan(r[lane + kWarp]));
         const float nxt = __shfl_down_sync(kFull, tv, 1);
-        const bool bad = (lane < K && !(tv > nxt)) || (lane == K && !(tv > -INFINITY));
+        const bool bad = (lane < K && !(tv > nxt)) || (lane == K && !(tv > -INFINITY)) || seed_nan;
         if (!__ballot_sync(kFull, bad)) {
             if (lane < K) h.idx[lane] = ti;
             __syncwarp();
@@ -518,7 +522,8 @@ eval_mf_kernel(const float* __restrict__ Utab, const float* __restrict__ Vtab, i
 // spread over its lanes (lane r = rank r; K+1 <= 32): an insertion is one ballot + two
 // shuffles instead of ~150 single-lane heap instructions.  At the end the warp checks that the
 // K+1 values are strictly decreasing and finite; users that fail the check (exact ties in the
-// top K+1, or fewer than K+1 unmasked items) are appended to a list and re-done by the exact
+// top K+1, fewer than K+1 unmasked items, or an unmasked NaN among the first L items, which the
+// reference's heap holds from the start) are appended to a list and re-done by the exact
 // heap-replay kernel above, so the result stays bit-identical to the reference for every input.
 // ----------------------------------------------------------------------------------------
 template <int TM, int TN, int kWarps>
@@ -554,6 +559,8 @@ eval_mf_fast_kernel(const float* __restrict__ Utab, const float* __restrict__ Vt
     float top_v[TM], thr[TM];   // lane r holds the rank-r entry of user m's running top-(K+1)
     int top_i[TM];
     bool live[TM];
+    const int L = (2 * K < N) ? 2 * K : N;   // the reference's heap size (evaluate.h:38)
+    unsigned seed_nan = 0u;                  // bit m: user m has an unmasked NaN score in [0, L)
 #pragma unroll
     for (int m = 0; m < TM; ++m) {
         const int b = user_slot0 + m;
@@ -633,6 +640,14 @@ eval_mf_fast_kernel(const float* __restrict__ Utab, const float* __restrict__ Vt
                 tr_pos[m] += c;
                 if (c < kWarp) break;
             }
+            if (base == 0) {   // the heap seed [0, L) lies in the first tile (L <= 62 < TILE)
+#pragma unroll
+                for (int n = 0; n < TN; ++n) {
+                    const int item = n * 32 + lane;
+                    if (__any_sync(kFull, item < L && !((maskbits[n] >> lane) & 1u) && isnan(acc[m][n])))
+                        seed_nan |= 1u << m;
+                }
+            }
 #pragma unroll
             for (int n = 0; n < TN; ++n) {
                 const int item = base + n * 32 + lane;
@@ -660,9 +675,11 @@ eval_mf_fast_kernel(const float* __restrict__ Utab, const float* __restrict__ Vt
     for (int m = 0; m < TM; ++m) {
         if (!live[m]) continue;
         const int b = user_slot0 + m;
-        // decidable without the heap: K+1 finite, strictly decreasing values
+        // decidable without the heap: K+1 finite, strictly decreasing values, and no NaN in the
+        // heap seed (the reference's heap comparisons with a NaN all fail, which reorders it)
         const float nxt = __shfl_down_sync(kFull, top_v[m], 1);
-        const bool bad = (lane < K && !(top_v[m] > nxt)) || (lane == K && !(top_v[m] > -INFINITY));
+        const bool bad = (lane < K && !(top_v[m] > nxt)) || (lane == K && !(top_v[m] > -INFINITY)) ||
+                         ((seed_nan >> m) & 1u);
         if (__ballot_sync(kFull, bad)) {
             if (lane == 0) slow_rows[atomicAdd(slow_count, 1)] = b;
             continue;
@@ -734,6 +751,66 @@ mean_rows_kernel(const float* __restrict__ a, int64_t rows, int cols, float* __r
     if (ty == 0 && c < cols) out[c] = __fdiv_rn(acc, (float)rows);
 }
 
+// A one-column matrix is contiguous along axis 0, and there numpy reduces with its pairwise_sum
+// (numpy/_core/src/umath/loops_utils.h.src), starting from 0: below 8 values in order, up to 128
+// values in 8 interleaved partial sums, above that split at an even multiple of 8 and add the halves.
+__device__ float np_pairwise_leaf(const float* __restrict__ a, int64_t n) {   // n <= 128
+    if (n < 8) {
+        float r = 0.0f;
+        for (int64_t i = 0; i < n; ++i) r = __fadd_rn(r, __ldg(a + i));
+        return r;
+    }
+    float r[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = __ldg(a + j);
+    int64_t i = 8;
+    for (; i < n - (n % 8); i += 8)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] = __fadd_rn(r[j], __ldg(a + i + j));
+    float res = __fadd_rn(__fadd_rn(__fadd_rn(r[0], r[1]), __fadd_rn(r[2], r[3])),
+                          __fadd_rn(__fadd_rn(r[4], r[5]), __fadd_rn(r[6], r[7])));
+    for (; i < n; ++i) res = __fadd_rn(res, __ldg(a + i));
+    return res;
+}
+
+// The split tree walked without recursion (a recursive kernel's stack would outgrow the default
+// per-thread limit on long columns): the left child first, each pending right child's length on an
+// explicit stack, a node's sum = left + right as numpy adds them.  Leaves are visited in order, so the
+// next subtree always starts where the last leaf ended.  Every split roughly halves n, so the depth
+// stays below log2(2^63 / 128) + 2 < 64 for any int64 n (a 768-byte stack frame).
+constexpr int kPairwiseDepth = 64;
+__device__ float np_pairwise_sum(const float* __restrict__ a, int64_t n) {
+    int64_t s_len[kPairwiseDepth];   // length of the pending right child; -1 once it runs
+    float s_left[kPairwiseDepth];    // the node's left sum, once known
+    int sp = 0;
+    int64_t off = 0, len = n;
+    for (;;) {
+        while (len > 128) {
+            int64_t half = len / 2;
+            half -= half % 8;
+            s_len[sp++] = len - half;
+            len = half;
+        }
+        float r = np_pairwise_leaf(a + off, len);
+        off += len;
+        for (;;) {
+            if (sp == 0) return r;
+            if (s_len[sp - 1] >= 0) {
+                s_left[sp - 1] = r;
+                len = s_len[sp - 1];
+                s_len[sp - 1] = -1;
+                break;
+            }
+            r = __fadd_rn(s_left[sp - 1], r);
+            --sp;
+        }
+    }
+}
+
+__global__ void mean_column_kernel(const float* __restrict__ a, int64_t rows, float* __restrict__ out) {
+    out[0] = __fdiv_rn(np_pairwise_sum(a, rows), (float)rows);
+}
+
 static int check_metrics(const int32_t* metric_host, int metric_num) {
     NRC_REQUIRE(metric_num >= 0 && metric_num <= kMaxMetrics, NRC_E_LIMIT,
                 "metric_num %d outside [0, %d]", metric_num, kMaxMetrics);
@@ -758,6 +835,11 @@ static int check_metrics(const int32_t* metric_host, int metric_num) {
     return upload_tables();
 }
 
+// nrc_eval_last_routes: [0] form of the last nrc_eval_mf, [1] fast pass and [2] warps per CTA of the
+// last eval_rows_kernel launch; -1 until a call has decided them.  Process-wide (a test hook), so with
+// several host threads it holds whichever thread launched last.
+static int32_t g_routes[3] = {-1, -1, -1};
+
 static int launch_rows(const float* scores, int N, int rows, int K, int L, const int64_t* tptr,
                        const int32_t* tidx, int M, float* results, int32_t* ranks, bool metrics,
                        cudaStream_t st) {
@@ -768,6 +850,8 @@ static int launch_rows(const float* scores, int N, int rows, int K, int L, const
     const size_t smem = (size_t)warps * stride_bytes;
     const int grid = (rows + warps - 1) / warps;
     const int fast = (K + 1 <= 32 && K < N && !g_force_exact) ? 1 : 0;
+    g_routes[1] = fast;
+    g_routes[2] = warps;
     if (metrics) {
         NRC_CUDA_CHECK(cudaFuncSetAttribute(eval_rows_kernel<true>,
                                             cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
@@ -937,6 +1021,13 @@ extern "C" int nrc_eval_last_undecided(int32_t* count_host) {
     return NRC_OK;
 }
 
+// Host bookkeeping of which kernel forms the last calls launched (see g_routes); no device work.
+extern "C" int nrc_eval_last_routes(int32_t* out) {
+    NRC_REQUIRE(out != nullptr, NRC_E_VALUE, "out is NULL");
+    for (int i = 0; i < 3; ++i) out[i] = g_routes[i];
+    return NRC_OK;
+}
+
 // Routes of the last nrc_eval_mf_tc call: users re-ranked by the candidate-list heap replay (ties) and users
 // re-ranked by the full-catalogue eval_mf_kernel (an overflowed candidate list in either pass).  The second
 // count lives on the device, so this synchronises.
@@ -988,6 +1079,7 @@ extern "C" int nrc_eval_mf(const float* user_table, const float* item_table, int
     const int grid = (num_eval_users + W * TM - 1) / (W * TM);
     const bool fast = (K + 1 <= 32) && !g_force_exact;
     if (!fast) {
+        g_routes[0] = 0;
         kern<<<grid, W * 32, smem, st>>>(user_table, item_table, dim, num_items, users, num_eval_users,
                                          train_indptr, train_indices, test_indptr, test_indices, K, L,
                                          metric_num, results, ranks, nullptr, nullptr);
@@ -1007,6 +1099,7 @@ extern "C" int nrc_eval_mf(const float* user_table, const float* item_table, int
         constexpr int TMs = 2;
         const size_t fsmem = ((size_t)W * TMs * D4 + (size_t)TN * 32 * (D4 + 4)) * 4 + (size_t)W * TMs * 4 * K * 4;
         const int fgrid = (num_eval_users + W * TMs - 1) / (W * TMs);
+        g_routes[0] = 1;
         eval_mf_fast_kernel<TMs, TN, W><<<fgrid, W * 32, fsmem, st>>>(
             user_table, item_table, dim, num_items, users, num_eval_users, train_indptr, train_indices,
             test_indptr, test_indices, K, metric_num, results, ranks, g_slow, g_slow + 1);
@@ -1016,6 +1109,7 @@ extern "C" int nrc_eval_mf(const float* user_table, const float* item_table, int
         const size_t fsmem4 = ((size_t)W * TM * D4 + (size_t)4 * 32 * (D4 + 4)) * 4 + (size_t)W * TM * 4 * K * 4;
         if (tn_pref == 4 && fsmem4 <= 200 * 1024) {
             const size_t fsmem = fsmem4;
+            g_routes[0] = 2;
             NRC_CUDA_CHECK(cudaFuncSetAttribute(eval_mf_fast_kernel<8, 4, 8>,
                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
             eval_mf_fast_kernel<TM, 4, W><<<grid, W * 32, fsmem, st>>>(
@@ -1023,6 +1117,7 @@ extern "C" int nrc_eval_mf(const float* user_table, const float* item_table, int
                 test_indptr, test_indices, K, metric_num, results, ranks, g_slow, g_slow + 1);
         } else {
             const size_t fsmem = ((size_t)W * TM * D4 + (size_t)TN * 32 * (D4 + 4)) * 4 + (size_t)W * TM * 4 * K * 4;
+            g_routes[0] = 3;
             eval_mf_fast_kernel<TM, TN, W><<<grid, W * 32, fsmem, st>>>(
                 user_table, item_table, dim, num_items, users, num_eval_users, train_indptr, train_indices,
                 test_indptr, test_indices, K, metric_num, results, ranks, g_slow, g_slow + 1);
@@ -1139,7 +1234,7 @@ eval_tc_finalize_kernel(const float* __restrict__ Utab, const float* __restrict_
                         const int64_t* __restrict__ test_ptr, const int32_t* __restrict__ test_idx,
                         const int32_t* __restrict__ cand, const int32_t* __restrict__ cand_cnt,
                         const float* __restrict__ cand_val, const float* __restrict__ margin, int nslots, int cap,
-                        int K, int M, int force_exact, float* __restrict__ results,
+                        int K, int L, int M, int force_exact, float* __restrict__ results,
                         int32_t* __restrict__ ranks, int32_t* __restrict__ slow_count,
                         int32_t* __restrict__ slow_rows, int32_t* __restrict__ und_count,
                         int32_t* __restrict__ und_rows) {
@@ -1215,6 +1310,16 @@ eval_tc_finalize_kernel(const float* __restrict__ Utab, const float* __restrict_
             const float s = keep ? tc_exact_score(su4, Vtab, item, D) : -INFINITY;
             insert_all(s, item, keep, tv, ti, thr);
         }
+    }
+    // A NaN among the L items that seed the reference's heap reorders it (no comparison with a NaN
+    // holds), and neither this selection nor the candidate passes see it: such users take the
+    // full-catalogue heap replay.  Masked seeds are not excluded here (-inf in the reference), which
+    // only sends a few more users to the exact replay.
+    bool seed_nan = false;
+    for (int j = lane; j < L; j += kWarp) seed_nan |= isnan(tc_exact_score(su4, Vtab, j, D));
+    if (__any_sync(kFull, seed_nan)) {
+        if (lane == 0) slow_rows[atomicAdd(slow_count, 1)] = row;
+        return;
     }
     const float nxt = __shfl_down_sync(kFull, tv, 1);
     const bool bad = (lane < K && !(tv > nxt)) || (lane == K && !(tv > -INFINITY));
@@ -1380,7 +1485,7 @@ extern "C" int nrc_eval_mf_tc(const float* user_table, const float* item_table, 
         const size_t smem = (size_t)warps * ((dim + 4 * K + 3) & ~3) * 4;
         eval_tc_finalize_kernel<<<(num_eval_users + warps - 1) / warps, warps * 32, smem, st>>>(
             user_table, item_table, dim, users, num_eval_users, test_indptr, test_indices, c0.cand, c0.cnt,
-            c0.scratch, c0.margin, c0.nslots, c0.cap, K, metric_num, g_force_exact ? 1 : 0, results, ranks, g_slow, g_slow + 1, g_und,
+            c0.scratch, c0.margin, c0.nslots, c0.cap, K, L, metric_num, g_force_exact ? 1 : 0, results, ranks, g_slow, g_slow + 1, g_und,
             g_und + 1);
         NRC_CUDA_CHECK(cudaGetLastError());
     }
@@ -1470,6 +1575,7 @@ eval_merge_kernel(const int32_t* __restrict__ cand_ids, const float* __restrict_
     int* rank = smem_i + warp * 4 * K;
     float sc[kMergePerLane];
     int id[kMergePerLane];
+    bool has_nan = false;
 #pragma unroll
     for (int q = 0; q < kMergePerLane; ++q) {
         const int c = q * 32 + lane;
@@ -1477,9 +1583,11 @@ eval_merge_kernel(const int32_t* __restrict__ cand_ids, const float* __restrict_
         sc[q] = ok ? cand_scores[(size_t)row * C + c] : -INFINITY;
         id[q] = ok ? cand_ids[(size_t)row * C + c] : INT32_MAX;
         if (sc[q] == -INFINITY) id[q] = INT32_MAX;        // masked / padding entries never win a tie
+        has_nan |= isnan(sc[q]);
     }
-    bool tie = false;
-    float prev = INFINITY;
+    // a NaN candidate is never picked, but the reference's heap may hold it: the order is not decided
+    bool tie = __any_sync(kFull, has_nan);
+    float prev = NAN;                                     // equals nothing: a lone +inf at rank 0 is no tie
     for (int r = 0; r <= K; ++r) {                        // K picks + one more to see a tie at the cut
         float bs = -INFINITY; int bi = INT32_MAX, bq = -1;
 #pragma unroll
@@ -1554,7 +1662,8 @@ extern "C" int nrc_eval_merge_candidates(const int32_t* cand_ids, const float* c
     if (num_rows <= 0) return NRC_OK;
     int warps = 8;
     while (warps > 1 && (size_t)warps * 4 * top_k * 4 > 96 * 1024) warps >>= 1;
-    const size_t smem = (size_t)warps * 4 * top_k * 4;
+    const size_t smem = (size_t)warps * 4 * top_k * 4;   // above 48 KB from top_k 385 on
+    NRC_CUDA_CHECK(cudaFuncSetAttribute(eval_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     eval_merge_kernel<<<(num_rows + warps - 1) / warps, warps * 32, smem, as_stream(stream)>>>(
         cand_ids, cand_scores, C, num_rows, test_indptr, test_indices, top_k, metric_num, results, ranks, tie_count);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -1565,6 +1674,11 @@ extern "C" int nrc_mean_rows(const float* results, int64_t num_rows, int32_t num
                              float* out, void* stream) {
     NRC_REQUIRE(num_cols >= 0 && num_rows >= 0, NRC_E_VALUE, "negative shape");
     if (num_cols == 0) return NRC_OK;
+    if (num_cols == 1) {   // one metric at top_k 1: numpy's pairwise order, one thread
+        mean_column_kernel<<<1, 1, 0, as_stream(stream)>>>(results, num_rows, out);
+        NRC_CUDA_CHECK(cudaGetLastError());
+        return NRC_OK;
+    }
     mean_rows_kernel<<<(num_cols + 31) / 32, 256, 0, as_stream(stream)>>>(results, num_rows, num_cols, out);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;

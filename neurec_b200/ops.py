@@ -178,13 +178,54 @@ def use_tensor_core_eval(n_items, dim, top_k, n_users):
 def eval_mf_auto(user_table, item_table, users, train_indptr, train_indices, test_indptr, test_indices,
                  metric, top_k, return_ranks=False):
     """eval_mf, with the score step on the tensor cores when the catalogue is large enough for the
-    candidate pass to pay off (results are bit-identical either way)."""
+    candidate pass to pay off, and materialised score rows when (dim, top_k) lie outside the fused
+    kernel's shared-memory envelope (results are bit-identical on every route)."""
     n_items, dim = item_table.shape
     if use_tensor_core_eval(n_items, dim, top_k, users.numel()):
         return eval_mf_tc(user_table, item_table, users, train_indptr, train_indices, test_indptr, test_indices,
                           metric, top_k, return_ranks)
-    return eval_mf(user_table, item_table, users, train_indptr, train_indices, test_indptr, test_indices,
-                   metric, top_k, return_ranks)
+    try:
+        return eval_mf(user_table, item_table, users, train_indptr, train_indices, test_indptr, test_indices,
+                       metric, top_k, return_ranks)
+    except _lib.NrcError as e:
+        if e.rc != _lib.NRC_E_LIMIT:
+            raise
+    return eval_mf_materialised(user_table, item_table, users, train_indptr, train_indices, test_indptr,
+                                test_indices, metric, top_k, return_ranks)
+
+
+EVAL_CHUNK_BYTES = 256 << 20   # score rows eval_mf_materialised holds at a time
+
+
+def eval_mf_materialised(user_table, item_table, users, train_indptr, train_indices, test_indptr, test_indices,
+                         metric, top_k, return_ranks=False):
+    """eval_mf in user chunks through materialised scores: nrc_mf_scores (the fused kernel's FMA chain)
+    -> nrc_mask_rows -> nrc_eval_score_matrix, so the results are the fused kernel's bit for bit.  It
+    takes every dim and top_k <= 512, at the cost of writing [chunk, num_items] scores to memory."""
+    n_items = item_table.shape[0]
+    B = users.numel()
+    chunk = max(1, EVAL_CHUNK_BYTES // (4 * n_items))
+    res, ranks = [], []
+    for a in range(0, B, chunk):
+        u = users[a:a + chunk]
+        s = mask_rows(mf_scores(user_table, item_table, u), u, train_indptr, train_indices)
+        # the batch rows' test sets as a CSR indexed by row, as nrc_eval_score_matrix reads it
+        beg = test_indptr[u.long()]
+        cnt = test_indptr[u.long() + 1] - beg
+        tp = torch.zeros(u.numel() + 1, dtype=torch.int64, device=u.device)
+        torch.cumsum(cnt, 0, out=tp[1:])
+        src = torch.repeat_interleave(beg - tp[:-1], cnt) + torch.arange(int(tp[-1]), device=u.device)
+        ti = test_indices[src].contiguous()
+        out = eval_score_matrix(s, tp, ti, metric, top_k, return_ranks)
+        res.append(out[0] if return_ranks else out)
+        if return_ranks:
+            ranks.append(out[1])
+    if B == 0:
+        m = _metric_arr(metric)
+        res = [torch.empty((0, len(m) * top_k), dtype=torch.float32, device=users.device)]
+        ranks = [torch.empty((0, top_k), dtype=torch.int32, device=users.device)]
+    res = torch.cat(res)
+    return (res, torch.cat(ranks)) if return_ranks else res
 
 
 def eval_tc_items_version(version):
@@ -262,6 +303,18 @@ def eval_last_undecided():
     n = ctypes.c_int32(0)
     check(_lib.load().nrc_eval_last_undecided(ctypes.byref(n)))
     return n.value
+
+
+EVAL_ROUTES = ("mf_form", "rows_fast", "rows_warps")
+
+
+def eval_last_routes():
+    """Kernel forms of the most recent evaluator launches (nrc_eval_last_routes) as {name: value}; -1 = none yet.
+    mf_form: 0 heap replay for every user, 1 fast pass with 2 users per warp, 2 fast pass on 128-item tiles,
+    3 fast pass on 64-item tiles (last eval_mf); rows_fast, rows_warps: the last score-matrix / arg-top-k launch."""
+    out = (ctypes.c_int32 * len(EVAL_ROUTES))()
+    check(_lib.load().nrc_eval_last_routes(out))
+    return dict(zip(EVAL_ROUTES, out))
 
 
 def mf_scores(user_table, item_table, users):

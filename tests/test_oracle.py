@@ -392,3 +392,35 @@ def test_adjacency_restatements_equal_the_reference_classes(ml100k):
     w = kat["ngcf_norm"]
     got = digest(tf_math.ngcf_adj(d["train_indptr"], d["train_indices"], nu, ni, "norm"))
     assert got == (w["nnz"], w["indptr_crc32"], w["indices_crc32"], w["data_crc32"])
+
+
+@pytest.mark.skipif(oracle.ref_lib() is None, reason="oracle/_ref (the compiled reference headers) is not built")
+@pytest.mark.parametrize("trial", range(12))
+def test_oracle_equals_reference_headers_on_non_finite_scores(trial):
+    """The oracle is the truth the GPU evaluator is held to for non-finite scores as well: on matrices with NaN
+    inside and outside the heap seed [0, L), +-inf, all -inf rows and empty truth rows, arg_topk and evaluate_matrix
+    equal the reference's compiled arg_topk.h / evaluate.h (libstdc++'s partial_sort_copy keeps a NaN that seeds
+    its heap, which reorders the ranking; a NaN offered later is never admitted)."""
+    rs = np.random.RandomState(700 + trial)
+    for _ in range(40):
+        B, N, K = 8, int(rs.randint(2, 400)), int(rs.randint(1, 40))
+        K = min(K, N)
+        L = min(2 * K, N)
+        S = rs.randn(B, N).astype(np.float32)
+        if trial % 2:
+            S = np.round(S * 2).astype(np.float32)          # ties
+        S[rs.rand(B, N) < 0.05] = np.inf
+        S[rs.rand(B, N) < 0.05] = -np.inf
+        lo, hi = [(0, N), (0, L), (L, N)][trial % 3]
+        for b in range(B):
+            if hi > lo:
+                S[b, rs.randint(lo, hi, size=rs.randint(1, 4))] = np.nan
+        S[0] = -np.inf                                      # a row with nothing finite
+        S[1, :L] = np.nan                                   # a NaN heap root
+        for k in (K, L):
+            assert np.array_equal(oracle.arg_topk(S, k), oracle.arg_topk(S, k, impl="reference"))
+        truth = [rs.choice(N, rs.randint(0, min(N, 5) + 1), replace=False) for _ in range(B)]
+        truth[2] = []
+        ip, ix = oracle.lists_to_csr(truth)
+        want = oracle.evaluate_matrix(S, ip, ix, ALL, K, impl="reference")
+        assert np.array_equal(oracle.evaluate_matrix(S, ip, ix, ALL, K), want, equal_nan=True)
