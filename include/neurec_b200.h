@@ -663,6 +663,25 @@ int nrc_lightgcn_train_epoch(const int64_t* indptr, const int32_t* indices, cons
                              float* grad_e0, float* work_a, float* work_b, float* step_loss2,
                              void* stream);
 
+/* Test hook of the graph kernels (it reports and changes nothing; every route is chosen by the shape).
+ * nrc_graph_last_routes: HOST bookkeeping of what the most recent calls decided, written when a call launches (a
+ * call that returns before launching leaves it as it was); one record per process.  out i32[9]; -1 = no such
+ * launch yet, or not decided by the last call of that group:
+ *   SpMM (the last nrc_spmm_csr product, also those inside the LightGCN / NGCF calls):
+ *   [0] 1 the fast kernel, 0 the exact (sequential) kernel;
+ *   [1] fast: lanes per gathered row G = dim / 4 (8, 16, 32); exact: columns per lane V = dim / 32 (1, 2, 4), or 0
+ *       for the generic form (any dim up to 256);
+ *   [2] 1 when the grid was capped at 8 CTAs per SM, so a CTA (fast) or warp (exact) handles more than one 8-row
+ *       unit or row (n_rows > 64 * SMs), else 0;
+ *   NGCF (the last nrc_ngcf_forward / nrc_ngcf_grad; a forward sets [4] and [5] to -1):
+ *   [3] most rows per warp of the layer forward kernel;
+ *   [4] most 32-row tiles per CTA of the layer backward kernel (dW / db accumulated across them);
+ *   [5] most triplets per warp of the BPR gradient kernel (0 for an empty batch);
+ *   SpectralCF (the last nrc_spectralcf_forward / nrc_spectralcf_grad; 0 = no such product, as with 0 layers;
+ *   a forward sets [7] and [8] to -1): number of K slices (gridDim.y) of
+ *   [6] the forward products A_hat . E_{k-1}; [7] the backward products A_hat^T . dS; [8] the products dW_k. */
+int nrc_graph_last_routes(int32_t* out);
+
 /* ======================================================================================
  * NGCF: dense part of the propagation layer (SURVEY.md 8f rank 1)
  * ==================================================================================== */

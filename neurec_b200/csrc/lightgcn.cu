@@ -22,10 +22,13 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "graph.cuh"
 #include "learner.cuh"
 #include "optim.cuh"
 
 namespace nrc {
+
+int32_t g_graph_routes[kGraphRoutes] = {-1, -1, -1, -1, -1, -1, -1, -1, -1};
 
 template <int V> struct VecT;
 template <> struct VecT<1> { using T = float; };
@@ -297,9 +300,14 @@ static int spmm_launch(const SpmmArgs& A, cudaStream_t st) {
     NRC_REQUIRE(A.dim > 0 && A.dim <= 256, NRC_E_LIMIT, "dim %d outside [1, 256]", A.dim);
     const int threads = 256;
     const int64_t cap = (int64_t)sm_count() * 8;
+    // both kernels need ceil(n_rows / 8) CTAs of 8 warps for one unit (fast) or one row (exact) per warp; beyond the
+    // cap a CTA walks several units, a warp several rows
+    g_graph_routes[kRouteSpmmCapped] = ((int64_t)A.n_rows + 7) / 8 > cap ? 1 : 0;
     if (!g_spmm_exact && (A.dim == 32 || A.dim == 64 || A.dim == 128)) {
         int64_t blocks = ((int64_t)A.n_rows + 7) / 8;
         if (blocks > cap) blocks = cap;
+        g_graph_routes[kRouteSpmmFast] = 1;
+        g_graph_routes[kRouteSpmmWidth] = A.dim / 4;
         static int un = -1;
         // 8 row loads in flight per warp by default (NRC_SPMM_UN=4: four)
         if (un < 0) { const char* e = getenv("NRC_SPMM_UN"); un = (e && atoi(e) == 4) ? 4 : 8; }
@@ -317,6 +325,8 @@ static int spmm_launch(const SpmmArgs& A, cudaStream_t st) {
     }
     int64_t blocks = ((int64_t)A.n_rows * 32 + threads - 1) / threads;
     if (blocks > cap) blocks = cap;
+    g_graph_routes[kRouteSpmmFast] = 0;
+    g_graph_routes[kRouteSpmmWidth] = (A.dim == 32 || A.dim == 64 || A.dim == 128) ? A.dim / 32 : 0;
     if (A.dim == 32) spmm_csr_kernel<1><<<(unsigned)blocks, threads, 0, st>>>(A);
     else if (A.dim == 64) spmm_csr_kernel<2><<<(unsigned)blocks, threads, 0, st>>>(A);
     else if (A.dim == 128) spmm_csr_kernel<4><<<(unsigned)blocks, threads, 0, st>>>(A);
@@ -379,6 +389,13 @@ using namespace nrc;
 // bit-identical to scipy / TF's CPU kernel (parity tests); 0 (default): the fast order.
 extern "C" int nrc_spmm_set_exact(int32_t on) {
     g_spmm_exact = on != 0;
+    return NRC_OK;
+}
+
+// Host bookkeeping of the routes the most recent graph calls launched (see the header); no device work.
+extern "C" int nrc_graph_last_routes(int32_t* out) {
+    NRC_REQUIRE(out != nullptr, NRC_E_VALUE, "NULL output");
+    for (int r = 0; r < kGraphRoutes; ++r) out[r] = g_graph_routes[r];
     return NRC_OK;
 }
 

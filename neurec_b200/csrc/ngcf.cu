@@ -25,6 +25,7 @@
 //                           one RED per weight entry and CTA at the end
 //   the remaining A_hat^T . dside is nrc_spmm_csr with its fused bias (dego + A^T dside).
 #include "common.cuh"
+#include "graph.cuh"
 #include "learner.cuh"
 #include "philox.cuh"
 
@@ -40,11 +41,16 @@ struct NgcfDev {
     int din[kNgcfMaxLayers], dout[kNgcfMaxLayers];
     int w_off[kNgcfMaxLayers];        // packed weights: W_gc [din, dout], b_gc [dout], W_bi, b_bi per layer
     int e_off[kNgcfMaxLayers + 1];    // column offset of each block in the concatenated table
-    int64_t m_off[kNgcfMaxLayers];    // offset of layer k's [N, dout] block in masks / z1 / z2 / hd
+    int64_t m_off[kNgcfMaxLayers];    // offset of layer k's [N, dout] block in the caller's packed masks
+    // Workspace blocks start on 16 bytes: side, dside and hd blocks are operands of the SpMM, whose float2 / float4
+    // forms need aligned rows (N * width floats is not a multiple of 4 for an odd N and an odd width).
+    int64_t a_off[kNgcfMaxLayers];    // offset of layer k's [N, dout] block in z1 / z2 / hd
     int64_t side_off[kNgcfMaxLayers]; // offset of layer k's [N, din] block in side / dside buffers
     int weights_size;
     int64_t act_floats, in_floats;
 };
+
+static int64_t round4(int64_t n) { return (n + 3) & ~(int64_t)3; }
 
 static int ngcf_make(NgcfDev& S, const nrc_ngcf_shape* sh) {
     NRC_REQUIRE(sh != nullptr, NRC_E_VALUE, "shape is NULL");
@@ -55,20 +61,25 @@ static int ngcf_make(NgcfDev& S, const nrc_ngcf_shape* sh) {
     S.n_nodes = sh->num_users + sh->num_items;
     S.n_layers = sh->n_layers; S.emb_dim = sh->emb_dim;
     int in = sh->emb_dim, woff = 0, eoff = sh->emb_dim;
-    int64_t moff = 0, soff = 0;
+    int64_t moff = 0, aoff = 0, soff = 0;
     S.e_off[0] = 0;
     for (int k = 0; k < kNgcfMaxLayers; ++k) {
-        if (k >= S.n_layers) { S.din[k] = S.dout[k] = S.w_off[k] = 0; S.e_off[k + 1] = eoff; S.m_off[k] = moff; S.side_off[k] = soff; continue; }
+        if (k >= S.n_layers) {
+            S.din[k] = S.dout[k] = S.w_off[k] = 0; S.e_off[k + 1] = eoff; S.m_off[k] = moff; S.a_off[k] = aoff;
+            S.side_off[k] = soff;
+            continue;
+        }
         const int out = sh->layers[k];
         NRC_REQUIRE(out >= 1 && out <= kNgcfMaxDim, NRC_E_LIMIT, "layer width %d outside [1, %d]", out, kNgcfMaxDim);
         S.din[k] = in; S.dout[k] = out;
         S.w_off[k] = woff; woff += 2 * (in * out + out);
         S.e_off[k + 1] = eoff; eoff += out;
         S.m_off[k] = moff; moff += (int64_t)S.n_nodes * out;
-        S.side_off[k] = soff; soff += (int64_t)S.n_nodes * in;
+        S.a_off[k] = aoff; aoff += round4((int64_t)S.n_nodes * out);
+        S.side_off[k] = soff; soff += round4((int64_t)S.n_nodes * in);
         in = out;
     }
-    S.weights_size = woff; S.d_total = eoff; S.act_floats = moff; S.in_floats = soff;
+    S.weights_size = woff; S.d_total = eoff; S.act_floats = aoff; S.in_floats = soff;
     return NRC_OK;
 }
 
@@ -323,6 +334,10 @@ static int grid_for(int64_t work_items, int per_block) {
     return blocks < 1 ? 1 : (int)blocks;
 }
 
+static int32_t per_worker(int64_t work_items, int64_t workers) {
+    return (int32_t)((work_items + workers - 1) / workers);
+}
+
 }  // namespace nrc
 
 using namespace nrc;
@@ -371,6 +386,8 @@ int forward_impl(const NgcfDev& S, const int64_t* indptr, const int32_t* indices
                  const int32_t* row_order, const float* e0, const float* weights, const float* masks, float keep,
                  float* all_emb, const Work& W, cudaStream_t st) {
     const int N = S.n_nodes;
+    g_graph_routes[kRouteNgcfFwdRows] = per_worker(N, (int64_t)grid_for(N, 8) * 8);
+    g_graph_routes[kRouteNgcfBwdTiles] = g_graph_routes[kRouteNgcfBprTriplets] = -1;
     ngcf_copy_e0_kernel<<<grid_for((int64_t)N * S.emb_dim, 256), 256, 0, st>>>(e0, all_emb, N, S.emb_dim, S.d_total);
     NRC_CUDA_CHECK(cudaGetLastError());
     const float* ego = e0;
@@ -379,12 +396,12 @@ int forward_impl(const NgcfDev& S, const int64_t* indptr, const int32_t* indices
         int rc = nrc_spmm_csr(indptr, indices, values, row_order, N, ego, S.din[k], nullptr, side, nullptr, 0.0f, st);
         if (rc) return rc;
         NgcfLayerArgs A{ego, side, weights + S.w_off[k], masks ? masks + S.m_off[k] : nullptr, keep,
-                        W.z1 + S.m_off[k], W.z2 + S.m_off[k], W.hd + S.m_off[k], W.sq + (int64_t)k * N,
+                        W.z1 + S.a_off[k], W.z2 + S.a_off[k], W.hd + S.a_off[k], W.sq + (int64_t)k * N,
                         all_emb, S.d_total, S.e_off[k + 1], N, S.din[k], S.dout[k]};
         const size_t smem = ((size_t)2 * S.din[k] * S.dout[k] + 2 * S.dout[k] + 8 * 2 * S.din[k]) * 4;
         ngcf_layer_fwd_kernel<<<grid_for(N, 8), 256, smem, st>>>(A);
         NRC_CUDA_CHECK(cudaGetLastError());
-        ego = W.hd + S.m_off[k];
+        ego = W.hd + S.a_off[k];
     }
     return NRC_OK;
 }
@@ -426,6 +443,10 @@ extern "C" int nrc_ngcf_grad(const nrc_ngcf_shape* shape, const int64_t* indptr,
     if (rc) return rc;
     if (!t_indptr) { t_indptr = indptr; t_indices = indices; t_values = values; t_row_order = row_order; }
     NRC_CUDA_CHECK(cudaMemsetAsync(grad_weights, 0, (size_t)S.weights_size * sizeof(float), st));
+    const int tiles = (N + kBwdRows - 1) / kBwdRows;
+    const int bwd_grid = tiles < sm_count() * 2 ? tiles : sm_count() * 2;
+    g_graph_routes[kRouteNgcfBprTriplets] = batch > 0 ? per_worker(batch, (int64_t)grid_for(batch, 8) * 8) : 0;
+    g_graph_routes[kRouteNgcfBwdTiles] = per_worker(tiles, bwd_grid);
     if (batch > 0) {
         ngcf_bpr_grad_kernel<<<grid_for(batch, 8), 256, 0, st>>>(all_emb, S.d_total, shape->num_users, users, pos_items,
                                                                 neg_items, batch, reg, grad_all, loss2);
@@ -434,9 +455,9 @@ extern "C" int nrc_ngcf_grad(const nrc_ngcf_shape* shape, const int64_t* indptr,
     const float* d_next = nullptr;
     float* pp[2] = {W.dnA, W.dnB};
     for (int k = S.n_layers - 1; k >= 0; --k) {
-        const float* ego = (k == 0) ? e0 : W.hd + S.m_off[k - 1];
+        const float* ego = (k == 0) ? e0 : W.hd + S.a_off[k - 1];
         NgcfBwdArgs A{grad_all, S.d_total, S.e_off[k + 1], d_next, ego, W.side + S.side_off[k], weights + S.w_off[k],
-                      masks ? masks + S.m_off[k] : nullptr, keep, W.z1 + S.m_off[k], W.z2 + S.m_off[k], W.hd + S.m_off[k],
+                      masks ? masks + S.m_off[k] : nullptr, keep, W.z1 + S.a_off[k], W.z2 + S.a_off[k], W.hd + S.a_off[k],
                       W.sq + (int64_t)k * N, W.dside + S.side_off[k], W.dego, grad_weights + S.w_off[k], N, S.din[k], S.dout[k]};
         const size_t smem = ((size_t)2 * S.din[k] * (S.dout[k] + 1) + (size_t)2 * kBwdRows * S.din[k] +
                              (size_t)2 * kBwdRows * S.dout[k]) * 4;
@@ -445,10 +466,7 @@ extern "C" int nrc_ngcf_grad(const nrc_ngcf_shape* shape, const int64_t* indptr,
             NRC_CUDA_CHECK(cudaFuncSetAttribute(ngcf_layer_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
             attr_done = true;
         }
-        const int tiles = (N + kBwdRows - 1) / kBwdRows;
-        int grid = sm_count() * 2;
-        if (grid > tiles) grid = tiles;
-        ngcf_layer_bwd_kernel<<<grid, 256, smem, st>>>(A);
+        ngcf_layer_bwd_kernel<<<bwd_grid, 256, smem, st>>>(A);
         NRC_CUDA_CHECK(cudaGetLastError());
         // d_ego (input of this layer) = dego + A_hat^T . dside
         float* out = pp[k & 1];

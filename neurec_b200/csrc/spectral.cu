@@ -16,6 +16,7 @@
 // 32 rows x n columns per CTA, K consumed in chunks of 32 through shared memory, each thread 4 rows x n/32 columns.
 // gridDim.y > 1 splits K over CTAs (the dW = S^T dZ reduction over all nodes) and adds with RED.
 #include "common.cuh"
+#include "graph.cuh"
 #include "optim.cuh"
 
 namespace nrc {
@@ -161,8 +162,9 @@ copy_block_kernel(const float* __restrict__ src, int64_t N, int d, int dtot, flo
     }
 }
 
+// route: the g_graph_routes entry that records this product's K split (gridDim.y), or -1
 static int gemm(const float* A, int64_t lda, int trans_a, const float* X, int64_t ldx, int trans_x, float* Y, int64_t ldy,
-                int M, int K, int n, int act, int split_k, cudaStream_t st) {
+                int M, int K, int n, int act, int split_k, int route, cudaStream_t st) {
     NRC_REQUIRE(n > 0 && n <= kGemmMaxN, NRC_E_LIMIT, "embedding_size %d outside [1, %d]", n, kGemmMaxN);
     GemmArgs G{A, lda, trans_a, X, ldx, trans_x, Y, ldy, M, K, n, act, K};
     unsigned gy = 1;
@@ -175,6 +177,7 @@ static int gemm(const float* A, int64_t lda, int trans_a, const float* X, int64_
         gy = (unsigned)((K + per - 1) / per);
         NRC_CUDA_CHECK(cudaMemset2DAsync(Y, (size_t)ldy * sizeof(float), 0, (size_t)n * sizeof(float), (size_t)M, st));
     }
+    if (route >= 0) g_graph_routes[route] = (int32_t)gy;
     dim3 grid((unsigned)((M + kGemmRows - 1) / kGemmRows), gy);
     dense_gemm_kernel<<<grid, 256, 0, st>>>(G);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -194,10 +197,12 @@ static int spectral_forward(int N, int d, int K, const float* a_hat, const float
     for (int k = 1; k <= K; ++k) {
         float* side = sides + (size_t)(k - 1) * N * d;
         // side = A_hat E_{k-1}   (E_{k-1} is the (k-1)-th column block of all_emb)
-        int rc = gemm(a_hat, N, 0, all_emb + (size_t)(k - 1) * d, dtot, 0, side, d, N, N, d, ACT_IDENTITY, 1, st);
+        int rc = gemm(a_hat, N, 0, all_emb + (size_t)(k - 1) * d, dtot, 0, side, d, N, N, d, ACT_IDENTITY, 1,
+                      kRouteSpecFwdSplit, st);
         if (rc) return rc;
         // E_k = act(side W_k)
-        rc = gemm(side, d, 0, filters + (size_t)(k - 1) * d * d, d, 0, all_emb + (size_t)k * d, dtot, N, d, d, act, 1, st);
+        rc = gemm(side, d, 0, filters + (size_t)(k - 1) * d * d, d, 0, all_emb + (size_t)k * d, dtot, N, d, d, act, 1, -1,
+                  st);
         if (rc) return rc;
     }
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -219,7 +224,11 @@ extern "C" int nrc_spectralcf_forward(int32_t num_nodes, int32_t dim, int32_t nu
                                       const float* e0, const float* filters, int32_t activation, float* all_emb,
                                       float* work, void* stream) {
     NRC_REQUIRE(num_nodes > 0 && dim > 0 && num_layers >= 0 && num_layers <= 8, NRC_E_VALUE, "bad SpectralCF shape");
+    // checked before the first launch: the layer-0 copy must not run for a width the products then reject
+    NRC_REQUIRE(dim <= kGemmMaxN, NRC_E_LIMIT, "embedding_size %d outside [1, %d]", dim, kGemmMaxN);
     NRC_REQUIRE(act_id(activation) >= 0, NRC_E_NOTIMPL, "ERROR");                        // tool.py:32-33
+    g_graph_routes[kRouteSpecFwdSplit] = 0;
+    g_graph_routes[kRouteSpecBwdSplit] = g_graph_routes[kRouteSpecDwSplit] = -1;
     return spectral_forward(num_nodes, dim, num_layers, a_hat, e0, filters, activation, all_emb, work, as_stream(stream));
 }
 
@@ -230,7 +239,9 @@ extern "C" int nrc_spectralcf_grad(int32_t num_users, int32_t num_items, int32_t
                                    float* grad_all, int32_t* touched, float* grad_e0, float* grad_filters, float* work,
                                    float* loss, void* stream) {
     NRC_REQUIRE(num_users > 0 && num_items > 0 && dim > 0 && num_layers >= 0 && num_layers <= 8, NRC_E_VALUE, "bad SpectralCF shape");
+    NRC_REQUIRE(dim <= kGemmMaxN, NRC_E_LIMIT, "embedding_size %d outside [1, %d]", dim, kGemmMaxN);
     NRC_REQUIRE(act_id(activation) >= 0, NRC_E_NOTIMPL, "ERROR");
+    g_graph_routes[kRouteSpecFwdSplit] = g_graph_routes[kRouteSpecBwdSplit] = g_graph_routes[kRouteSpecDwSplit] = 0;
     cudaStream_t st = as_stream(stream);
     const int N = num_users + num_items, d = dim, K = num_layers, dtot = d * (K + 1);
     float* sides = work;
@@ -252,13 +263,14 @@ extern "C" int nrc_spectralcf_grad(int32_t num_users, int32_t num_items, int32_t
         const float* side = sides + (size_t)(k - 1) * N * d;
         const float* W = filters + (size_t)(k - 1) * d * d;
         // dW_k = side^T dZ   (reduction over all N nodes: split over CTAs)
-        rc = gemm(side, d, 1, dZ, d, 0, grad_filters + (size_t)(k - 1) * d * d, d, d, N, d, ACT_IDENTITY, 64, st);
+        rc = gemm(side, d, 1, dZ, d, 0, grad_filters + (size_t)(k - 1) * d * d, d, d, N, d, ACT_IDENTITY, 64,
+                  kRouteSpecDwSplit, st);
         if (rc) return rc;
         // dS = dZ W_k^T
-        rc = gemm(dZ, d, 0, W, d, 1, dS, d, N, d, d, ACT_IDENTITY, 1, st);
+        rc = gemm(dZ, d, 0, W, d, 1, dS, d, N, d, d, ACT_IDENTITY, 1, -1, st);
         if (rc) return rc;
         // carry = A_hat^T dS
-        rc = gemm(at, N, at_trans, dS, d, 0, carry, d, N, N, d, ACT_IDENTITY, 1, st);
+        rc = gemm(at, N, at_trans, dS, d, 0, carry, d, N, N, d, ACT_IDENTITY, 1, kRouteSpecBwdSplit, st);
         if (rc) return rc;
         have_carry = true;
     }

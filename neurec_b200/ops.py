@@ -554,6 +554,18 @@ def spmm_csr(indptr, indices, values, x, row_order=None, bias=None, y=None, sum_
     return y
 
 
+GRAPH_ROUTES = ("spmm_fast", "spmm_width", "spmm_capped", "ngcf_fwd_rows", "ngcf_bwd_tiles", "ngcf_bpr_triplets",
+                "spectral_fwd_split", "spectral_bwd_split", "spectral_dw_split")
+
+
+def graph_last_routes():
+    """Routes of the most recent SpMM / NGCF / SpectralCF launches (nrc_graph_last_routes) as {name: value}; -1 = no
+    such launch yet or not decided by the last call of that group."""
+    out = (ctypes.c_int32 * len(GRAPH_ROUTES))()
+    check(_lib.load().nrc_graph_last_routes(out))
+    return dict(zip(GRAPH_ROUTES, out))
+
+
 def lightgcn_propagate(indptr, indices, values, row_order, e0, n_layers, e_final=None, work=None):
     """mean(E_0, A E_0, ..., A^L E_0) (LightGCN.py:132-149)."""
     n, dim = e0.shape
