@@ -467,6 +467,27 @@ int nrc_mf_bpr_sgd_epoch_hot(float* user_table, float* const* item_shards, int32
 /* hot[e] += hot_delta[e]; hot_delta[e] = 0 for e < n_floats (a multiple of 4; both 16-byte aligned). */
 int nrc_mf_hot_apply(float* hot, float* hot_delta, int64_t n_floats, void* stream);
 
+/* Test hook of the MF training kernels (it reports and changes nothing; every route is chosen by the shape).
+ * nrc_mf_last_routes: HOST bookkeeping of the most recent launch of each kernel group, written when a call launches
+ * (a call that returns before launching, for a failed check or an empty batch, leaves it as it was); one record per
+ * process.  out i32[6 * 7], group k at out[7 * k]; -1 = no such launch yet, or a field the group does not decide.
+ *   groups: [0] nrc_mf_pairwise_grad / _pointwise_grad (also inside nrc_mf_train_epoch / _train_step_host);
+ *   [1] the id-fed in-place step (nrc_mf_bpr_sgd_fused / _sharded); [2] the CSR-fed in-place step
+ *   (nrc_mf_bpr_sgd_epoch / _epoch_hot); [3] nrc_mf_bpr_lazy_adam_epoch; [4] the persistent nrc_mf_epoch_fused;
+ *   [5] the multi-tensor optimizer apply (nrc_opt_apply_rows / _multi and the second phase of the per-step paths).
+ *   fields of a group:
+ *   +0 VEC, floats per lane of a row (dim / 32 for dim 32, 64, 128), 0 the generic any-dim loop;
+ *   +1 1 when the kernel's SHARDED form ran (item rows addressed through the shard table), else 0;
+ *   +2 CSR-fed step: 1 when user rows touched once by the launch take a plain store (pos_items == train_indices);
+ *   +3 CSR-fed step: head rows held in the shared-memory tier, min(n_hot, 8192 / dim);
+ *   +4 CTAs launched;
+ *   +5 1 when the grid was capped, so a warp (or thread) takes more than one triplet, sample or element: grad and
+ *      id-fed step above 64 * SMs triplets, CSR-fed step above 768 per resident CTA, lazy Adam above 2048 * SMs,
+ *      persistent epoch when a batch of the launch exceeds its 16 * SMs warps, optimizer apply above 2048 * SMs
+ *      elements; else 0;
+ *   +6 persistent epoch: 1 the float4 optimizer pass (dim % 4 == 0), 0 the per-element one. */
+int nrc_mf_last_routes(int32_t* out);
+
 
 /* The explicitly-named LAZY-Adam variant of nrc_mf_bpr_sgd_epoch (SURVEY.md 8d, BASELINE configs[4]:
  * "learner=gd for the roofline run plus an explicitly-named lazy-Adam run"; the reference's own

@@ -22,6 +22,7 @@
 // kernel launches and their gaps.
 #include "epoch.cuh"
 #include "mf.cuh"
+#include "mf_routes.cuh"
 #include "optim.cuh"
 
 #include <cooperative_groups.h>
@@ -317,6 +318,10 @@ extern "C" int nrc_mf_epoch_fused(float* user_table, float* item_table, int32_t 
     int per_sm = 0;
     NRC_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 512, 0));
     NRC_REQUIRE(per_sm >= 1, NRC_E_CUDA, "the persistent epoch kernel does not fit an SM");
+    // capped: the largest batch of the launch has more samples than the grid has warps (phase 1 loops)
+    const int64_t rest = P.n_used - first_step * batch_size, most = rest < batch_size ? rest : batch_size;
+    mf_route(kMfEpoch, dim == 128 ? 4 : dim == 64 ? 2 : dim == 32 ? 1 : 0, 0, -1, -1, sm_count(),
+             most > (int64_t)sm_count() * (512 / 32), (dim & 3) == 0 ? 1 : 0);
     void* args[] = {&P};
     NRC_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(sm_count()), dim3(512), args, 0, st));
     return NRC_OK;

@@ -20,6 +20,8 @@
 // same gradient).
 #include "optim.cuh"
 
+#include "mf_routes.cuh"
+
 namespace nrc {
 
 struct OptParams {
@@ -91,7 +93,9 @@ int opt_launch_run(const OptLaunch& L, int32_t stamp, cudaStream_t st) {
     P.stamp = stamp; P.total = L.total;
     int64_t blocks = (L.total + 255) / 256;
     const int64_t cap = (int64_t)sm_count() * 8;
+    const bool capped = blocks > cap;
     if (blocks > cap) blocks = cap;
+    mf_route(kMfOptApply, -1, -1, -1, -1, blocks, capped, -1);
     opt_apply_kernel<<<(unsigned)blocks, 256, 0, st>>>(P);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;

@@ -22,9 +22,14 @@
 #include "epoch.cuh"
 #include "learner.cuh"
 #include "mf.cuh"
+#include "mf_routes.cuh"
 #include "optim.cuh"
 
 namespace nrc {
+
+int32_t g_mf_routes[kMfKernels][kMfFields] = {{-1, -1, -1, -1, -1, -1, -1}, {-1, -1, -1, -1, -1, -1, -1},
+                                              {-1, -1, -1, -1, -1, -1, -1}, {-1, -1, -1, -1, -1, -1, -1},
+                                              {-1, -1, -1, -1, -1, -1, -1}, {-1, -1, -1, -1, -1, -1, -1}};
 
 // Phase 1 of a step: one warp per triplet (PAIRWISE: third = negative items) or sample (third = labels' bits).
 // The any-dim form of mf_sample_grad, ordinary loads.
@@ -170,11 +175,13 @@ static int launch_bpr_sgd(const RowShards& SU, const RowShards& SV, int dim, con
                           cudaStream_t st) {
     int64_t blocks = (batch + 7) / 8;
     const int64_t cap = (int64_t)sm_count() * 8;   // 8 resident CTAs of 256 threads per SM
+    const bool capped = blocks > cap;
     if (blocks > cap) blocks = cap;
     const unsigned gb = (unsigned)blocks;
 #define NRC_LAUNCH_SGD(VEC, SH) \
     mf_bpr_sgd_fused_kernel<VEC, SH><<<gb, 256, 0, st>>>(SU, SV, users, pos, neg, batch, lr, reg, loss)
     const bool sharded = SU.rows_per_shard != 0;
+    mf_route(kMfSgdIds, dim == 128 ? 4 : dim == 64 ? 2 : 1, sharded, -1, -1, blocks, capped, -1);
     if (dim == 128) { if (sharded) NRC_LAUNCH_SGD(4, true); else NRC_LAUNCH_SGD(4, false); }
     else if (dim == 64) { if (sharded) NRC_LAUNCH_SGD(2, true); else NRC_LAUNCH_SGD(2, false); }
     else { if (sharded) NRC_LAUNCH_SGD(1, true); else NRC_LAUNCH_SGD(1, false); }
@@ -386,7 +393,10 @@ static int launch_stream(float* U_local, const RowShards& SV, const EpochSpec& E
         grid_cap = (int64_t)per_sm * sm_count();
     }
     int64_t blocks = (count + kStreamThreads - 1) / kStreamThreads;
+    const bool capped = blocks > grid_cap;
     if (blocks > grid_cap) blocks = grid_cap;
+    mf_route(kMfSgdCsr, VEC, SH, user_once, SV.n_hot < kSgdTierRows<VEC> ? SV.n_hot : kSgdTierRows<VEC>, blocks, capped,
+             -1);
     mf_bpr_sgd_stream_kernel<VEC, SH><<<(unsigned)blocks, kStreamThreads, smem, st>>>(U_local, SV, E, first, count,
                                                                                       user_once, lr, reg, loss);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -511,6 +521,7 @@ extern "C" int nrc_mf_pairwise_grad(const float* user_table, const float* item_t
                 NRC_E_VALUE, "please choose a suitable loss function");
     NRC_REQUIRE(dim > 0 && batch >= 0, NRC_E_VALUE, "dim must be positive, batch >= 0");
     if (batch == 0) return NRC_OK;
+    mf_route(kMfGrad, 0, 0, -1, -1, grad_grid(batch), (batch + 7) / 8 > (int64_t)sm_count() * 8, -1);
     mf_grad_kernel<true><<<grad_grid(batch), 256, 0, as_stream(stream)>>>(
         user_table, item_table, dim, users, pos_items, neg_items, batch, loss_kind, reg, grad_user,
         grad_item, touched_user, touched_item, stamp, loss);
@@ -529,6 +540,7 @@ extern "C" int nrc_mf_pointwise_grad(const float* user_table, const float* item_
                 "please choose a suitable loss function");
     NRC_REQUIRE(dim > 0 && batch >= 0, NRC_E_VALUE, "dim must be positive, batch >= 0");
     if (batch == 0) return NRC_OK;
+    mf_route(kMfGrad, 0, 0, -1, -1, grad_grid(batch), (batch + 7) / 8 > (int64_t)sm_count() * 8, -1);
     mf_grad_kernel<false><<<grad_grid(batch), 256, 0, as_stream(stream)>>>(
         user_table, item_table, dim, users, items, reinterpret_cast<const int32_t*>(labels), batch, loss_kind, reg,
         grad_user, grad_item, touched_user, touched_item, stamp, loss);
@@ -682,13 +694,23 @@ extern "C" int nrc_mf_bpr_lazy_adam_epoch(float* user_table, float* user_m, floa
     if (count == 0) return NRC_OK;
     int64_t blocks = (count + 255) / 256;
     const int64_t cap = (int64_t)sm_count() * 8;
+    const bool capped = blocks > cap;
     if (blocks > cap) blocks = cap;
+    mf_route(kMfLazyAdam, dim / 32, 0, -1, -1, blocks, capped, -1);
     cudaStream_t st = as_stream(stream);
 #define NRC_LAZY(VEC) mf_bpr_lazy_adam_stream_kernel<VEC><<<(unsigned)blocks, 256, 0, st>>>( \
         user_table, user_m, user_v, item_table, item_m, item_v, E, first, count, lr_t, beta1, beta2, eps, reg, loss)
     if (dim == 128) NRC_LAZY(4); else if (dim == 64) NRC_LAZY(2); else NRC_LAZY(1);
 #undef NRC_LAZY
     NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+// Host bookkeeping of the routes the most recent MF training launches took (see the header); no device work.
+extern "C" int nrc_mf_last_routes(int32_t* out) {
+    NRC_REQUIRE(out != nullptr, NRC_E_VALUE, "out is NULL");
+    for (int k = 0; k < kMfKernels; ++k)
+        for (int f = 0; f < kMfFields; ++f) out[k * kMfFields + f] = g_mf_routes[k][f];
     return NRC_OK;
 }
 

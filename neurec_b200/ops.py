@@ -498,6 +498,19 @@ def mf_bpr_lazy_adam_epoch(U, mU, vU, V, mV, vV, train_indptr, train_indices, po
     _count()
 
 
+MF_KERNELS = ("grad", "sgd_ids", "sgd_csr", "lazy_adam", "epoch", "opt_apply")
+MF_ROUTE_FIELDS = ("vec", "sharded", "user_once", "tier_rows", "grid", "capped", "opt_vec4")
+
+
+def mf_last_routes():
+    """Routes of the most recent launch of each MF training kernel group (nrc_mf_last_routes) as
+    {kernel: {field: value}}; -1 = no such launch yet or a field the group does not decide."""
+    nf = len(MF_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(MF_KERNELS) * nf))()
+    check(_lib.load().nrc_mf_last_routes(out))
+    return {k: dict(zip(MF_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(MF_KERNELS)}
+
+
 def opt_apply_rows(opt, var, grad, slot0, slot1, touched, stamp, hyper):
     h = np.zeros(4, dtype=np.float32)
     h[:len(hyper)] = hyper
