@@ -865,6 +865,87 @@ int nrc_wrmf_half_step(const float* fixed, int32_t num_fixed, const int64_t* ind
                        const int32_t* row_order, int32_t num_rows, int32_t dim, float alpha, float reg, float* out,
                        float* work, int32_t* not_spd, void* stream);
 
+/* ======================================================================================
+ * Sequential recommenders: FPMC and TransRec (model/sequential_recommender/), high_order = 1
+ * ==================================================================================== */
+
+/* Shared conventions.  One batch is (users, recent, items, third) i32 [batch] each, with `third` the negatives (i32,
+ * pairwise = 1) or the labels (f32, pairwise = 0) -- the layout of TimeOrderPairwiseSampler / TimeOrderPointwiseSampler
+ * (data/sampler.py:216-354).  Losses are learner.pairwise_loss / pointwise_loss (util/learner.py:17-41); the batch
+ * loss is ADDED into *loss; row gradients are ADDED into dense accumulators (duplicate ids sum, as TF's IndexedSlices
+ * de-duplication does) and every row that receives one gets `stamp` in its touched array (the rows adagrad, momentum
+ * and rmsprop move).  NRC_E_LIMIT when dim is outside [1, 256]; NRC_E_VALUE with "please choose a suitable loss
+ * function" for a loss the mode does not define.  A rejected call writes nothing. */
+
+/* FPMC._create_inference / _create_loss, FPMC.py:61-84, tables UI [U, d], IU, IL, LI [I, d]:
+ *   x(u, l, i) = <UI_u, IU_i> + <IL_i, LI_l>     (l = the recent item)
+ *   pairwise   l(x_i - x_j) + reg * l2_loss(UI_u, IU_i, IL_i, LI_l, IU_j, IL_j)
+ *   pointwise  l(z, x_i)    + reg * l2_loss(UI_u, IU_i, IL_i, LI_l)
+ * touched_user <- users, touched_item <- items and negatives (IU and IL), touched_recent <- recent (LI). */
+int nrc_fpmc_grad(const float* ui, const float* iu, const float* il, const float* li, int32_t dim,
+                  const int32_t* users, const int32_t* recent, const int32_t* items, const void* third,
+                  int64_t batch, int32_t pairwise, int32_t loss_kind, float reg, float* grad_ui,
+                  float* grad_iu, float* grad_il, float* grad_li, int32_t* touched_user,
+                  int32_t* touched_item, int32_t* touched_recent, int32_t stamp, float* loss, void* stream);
+
+/* FPMC.train_model's batch loop, FPMC.py:106-131, over a device-built epoch of n samples: per batch nrc_fpmc_grad +
+ * one TF-1.12 optimizer launch over UI, IU, IL and LI.  slot0 / slot1: HOST arrays of the four variables' slot
+ * pointers in that order (NULL where the optimizer keeps no such slot); lr_t_host f32 [steps] (adam), hyper_host
+ * as nrc_opt_apply_rows; step_loss f32 [steps] receives every batch's loss; stamps first_stamp .. + steps - 1. */
+int nrc_fpmc_train_epoch(float* ui, float* iu, float* il, float* li, int32_t num_users, int32_t num_items,
+                         int32_t dim, const int32_t* users, const int32_t* recent, const int32_t* items,
+                         const void* third, int64_t n, int32_t batch_size, int32_t pairwise, int32_t loss_kind,
+                         float reg, int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                         float* grad_ui, float* grad_iu, float* grad_il, float* grad_li,
+                         int32_t* touched_user, int32_t* touched_item, int32_t* touched_recent,
+                         float* const* slot0, float* const* slot1, int32_t first_stamp, float* step_loss,
+                         void* stream);
+
+/* FPMC.predict, FPMC.py:140-165: out f32 [rows, num_items], out[r, j] = <UI_u, IU_j> + <IL_j, LI_l> for
+ * (u, l) = (users[r], recent[r]). */
+int nrc_fpmc_scores(const float* ui, const float* iu, const float* il, const float* li, int32_t num_items,
+                    int32_t dim, const int32_t* users, const int32_t* recent, int64_t rows, float* out,
+                    void* stream);
+
+/* Scratch of nrc_transrec_grad / nrc_transrec_train_epoch in floats: per-CTA partial sums of g's gradient and a
+ * completion counter.  Zero-fill it once before its first use; every call leaves it ready for the next (calls that
+ * share one work buffer must not run concurrently). */
+int64_t nrc_transrec_work_floats(int32_t dim);
+
+/* TransRec._create_inference / _create_loss, TransRec.py:66-91, variables P [U, d], Q [I, d], b [I], g [1, d]:
+ *   x(u, l, i) = b_i - |(P_u + g) + Q_l - Q_i|^2          (squared)
+ *   pairwise   l(x_i - x_j) + reg * l2_loss(P_u, Q_l, Q_j, Q_i, b_i, b_j, g)
+ *   pointwise  l(z, x_i)    + reg * l2_loss(P_u, Q_l, Q_i, b_i, g)
+ * g's reg term enters once per batch.  grad_global f32 [d] is a dense gradient: it is summed per CTA and then across
+ * CTAs in one fixed order (no per-sample atomics) and added into grad_global.  touched_user <- users,
+ * touched_item <- recent, items and negatives (Q), touched_bias <- items and negatives only (b). */
+int nrc_transrec_grad(const float* user_table, const float* item_table, const float* item_bias,
+                      const float* global, int32_t dim, const int32_t* users, const int32_t* recent,
+                      const int32_t* items, const void* third, int64_t batch, int32_t pairwise,
+                      int32_t loss_kind, float reg, float* grad_user, float* grad_item, float* grad_bias,
+                      float* grad_global, int32_t* touched_user, int32_t* touched_item,
+                      int32_t* touched_bias, int32_t stamp, float* work, float* loss, void* stream);
+
+/* TransRec.train_model's batch loop, TransRec.py:110-147: per batch nrc_transrec_grad + one optimizer launch over P,
+ * Q, b (IndexedSlices rules) and g (dense rules: Adam and RMSProp take the Apply* formulas).  slot0 / slot1: HOST
+ * arrays of the four variables' slot pointers in the order P, Q, b, g; the rest as nrc_fpmc_train_epoch. */
+int nrc_transrec_train_epoch(float* user_table, float* item_table, float* item_bias, float* global,
+                             int32_t num_users, int32_t num_items, int32_t dim, const int32_t* users,
+                             const int32_t* recent, const int32_t* items, const void* third, int64_t n,
+                             int32_t batch_size, int32_t pairwise, int32_t loss_kind, float reg,
+                             int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                             float* grad_user, float* grad_item, float* grad_bias, float* grad_global,
+                             int32_t* touched_user, int32_t* touched_item, int32_t* touched_bias,
+                             float* const* slot0, float* const* slot1, int32_t first_stamp, float* work,
+                             float* step_loss, void* stream);
+
+/* TransRec's prediction graph, TransRec.py:102-107: out f32 [rows, num_items],
+ * out[r, j] = b_j - sqrt(sum_k (x_k - Q_jk)^2) with x = (P_u + g) + Q_l -- the distance, NOT squared.  The sum is
+ * taken over the differences themselves, so x == Q_j scores exactly b_j. */
+int nrc_transrec_scores(const float* user_table, const float* item_table, const float* item_bias,
+                        const float* global, int32_t num_items, int32_t dim, const int32_t* users,
+                        const int32_t* recent, int64_t rows, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,14 +22,15 @@ random.seed(2018)         # main.py:11  (tf.set_random_seed(2017) -> model init 
 
 
 def resolve_model(recommender):
-    # main.py:30-40: general_recommender first, then social_recommender; only the embedding-BPR family is on the
-    # accelerated hot path
-    for family in ("general_recommender", "social_recommender"):
+    # main.py:30-40: general_recommender first, then social_recommender, then sequential_recommender; only the models
+    # listed below are on the accelerated hot path
+    for family in ("general_recommender", "social_recommender", "sequential_recommender"):
         name = "neurec_b200.model.%s.%s" % (family, recommender)
         if importlib.util.find_spec(name) is not None:
             return getattr(importlib.import_module(name), recommender)
     raise ImportError("recommender '%s' is outside the accelerated hot path "
-                      "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, WRMF, SBPR)" % recommender)
+                      "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, WRMF, SBPR, FPMC, TransRec)"
+                      % recommender)
 
 
 if __name__ == "__main__":

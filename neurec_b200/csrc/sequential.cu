@@ -1,0 +1,484 @@
+// The sequential recommenders that score with embedding tables: FPMC and TransRec, fed by the time-ordered samplers
+// at high_order = 1 (one recent item per sample).
+//
+// Replaces (reference paths):
+//   model/sequential_recommender/FPMC.py:61-84       _create_inference / _create_loss (four tables, pairwise / pointwise)
+//   model/sequential_recommender/FPMC.py:97-134      train_model's batch loop (sess.run((loss, optimizer)) per batch)
+//   model/sequential_recommender/FPMC.py:140-165     predict
+//   model/sequential_recommender/TransRec.py:66-91   _create_inference / _create_loss (squared translation distance)
+//   model/sequential_recommender/TransRec.py:110-147 train_model's batch loop
+//   model/sequential_recommender/TransRec.py:102-107,153-166  prediction graph (Euclidean distance, not squared)
+//
+// Neither score is the inner product of one user row and one item row, so neither goes through the MF kernels:
+//   FPMC       x(u, l, i) = <UI_u, IU_i> + <IL_i, LI_l>
+//   TransRec   x(u, l, i) = b_i - |(P_u + g) + Q_l - Q_i|^2          (training)
+//              s(u, l, j) = b_j - |(P_u + g) + Q_l - Q_j|             (prediction)
+// Both gradient kernels run one warp per sample and add row gradients into dense accumulators with atomics (duplicate
+// ids sum, as TF's IndexedSlices de-duplication does).  TransRec's global vector g enters every sample; its gradient
+// is summed per warp, then per CTA in warp order, then across CTAs in CTA order by the last CTA to finish -- a fixed
+// order for a given batch size, and no atomics onto the same d floats.
+#include "common.cuh"
+#include "learner.cuh"
+#include "optim.cuh"
+
+namespace nrc {
+
+constexpr int kSeqMaxDim = 256;
+constexpr int kSeqPerLane = kSeqMaxDim / kWarp;   // row elements one lane holds at the widest dim
+constexpr int kSeqWarps = 8;                      // warps of a 256-thread CTA
+constexpr int kTransRecCtas = 128;                // TransRec gradient grid cap: work holds one partial g per CTA
+constexpr int kScoreRows = 8;                     // score kernels: (user, recent) rows per CTA
+
+static unsigned seq_grad_grid(int64_t batch, int64_t cap) {
+    int64_t blocks = (batch + kSeqWarps - 1) / kSeqWarps;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    return (unsigned)blocks;
+}
+
+// ---------------------------------------------------------------------------------------------
+// FPMC (FPMC.py:61-84).  c = dl/dx;
+//   pairwise   x = x_i - x_j, reg * l2_loss(UI_u, IU_i, IL_i, LI_l, IU_j, IL_j)
+//   pointwise  x = x_i,       reg * l2_loss(UI_u, IU_i, IL_i, LI_l)
+// ---------------------------------------------------------------------------------------------
+template <bool PAIRWISE>
+__global__ void __launch_bounds__(256)
+fpmc_grad_kernel(const float* __restrict__ UI, const float* __restrict__ IU, const float* __restrict__ IL,
+                 const float* __restrict__ LI, int D, const int32_t* __restrict__ users, const int32_t* __restrict__ recent,
+                 const int32_t* __restrict__ items, const void* __restrict__ third, int64_t batch, int loss_kind, float reg,
+                 float inv_b, float* __restrict__ gUI, float* __restrict__ gIU, float* __restrict__ gIL,
+                 float* __restrict__ gLI, int32_t* __restrict__ tU, int32_t* __restrict__ tI, int32_t* __restrict__ tL,
+                 int32_t stamp, float* __restrict__ loss) {
+    const int lane = threadIdx.x & 31;
+    const int64_t wpb = blockDim.x >> 5;
+    float loss_acc = 0.0f;
+    for (int64_t b = blockIdx.x * wpb + (threadIdx.x >> 5); b < batch; b += (int64_t)gridDim.x * wpb) {
+        const int u = users[b], l = recent[b], i = items[b];
+        const int j = PAIRWISE ? static_cast<const int32_t*>(third)[b] : 0;
+        const size_t ou = (size_t)u * D, ol = (size_t)l * D, oi = (size_t)i * D, oj = (size_t)j * D;
+        float xi = 0.f, xj = 0.f, sq = 0.f;
+        for (int t = lane; t < D; t += kWarp) {
+            const float a = UI[ou + t], ui = IU[oi + t], li = IL[oi + t], r = LI[ol + t];
+            xi = fmaf(a, ui, xi); xi = fmaf(li, r, xi);
+            sq += a * a + ui * ui + li * li + r * r;
+            if (PAIRWISE) {
+                const float uj = IU[oj + t], lj = IL[oj + t];
+                xj = fmaf(a, uj, xj); xj = fmaf(lj, r, xj);
+                sq += uj * uj + lj * lj;
+            }
+        }
+        xi = warp_sum(xi);
+        float lo, c;
+        if (PAIRWISE) pairwise_loss_grad(loss_kind, xi - warp_sum(xj), lo, c);
+        else pointwise_loss_grad(loss_kind, xi, static_cast<const float*>(third)[b], inv_b, lo, c);
+        if (reg != 0.0f) lo += reg * 0.5f * warp_sum(sq);
+        loss_acc += lo;
+        for (int t = lane; t < D; t += kWarp) {
+            const float a = UI[ou + t], ui = IU[oi + t], li = IL[oi + t], r = LI[ol + t];
+            if (PAIRWISE) {
+                const float uj = IU[oj + t], lj = IL[oj + t];
+                atomicAdd(gUI + ou + t, c * (ui - uj) + reg * a);
+                atomicAdd(gIU + oi + t, c * a + reg * ui);
+                atomicAdd(gIU + oj + t, -c * a + reg * uj);
+                atomicAdd(gIL + oi + t, c * r + reg * li);
+                atomicAdd(gIL + oj + t, -c * r + reg * lj);
+                atomicAdd(gLI + ol + t, c * (li - lj) + reg * r);
+            } else {
+                atomicAdd(gUI + ou + t, c * ui + reg * a);
+                atomicAdd(gIU + oi + t, c * a + reg * ui);
+                atomicAdd(gIL + oi + t, c * r + reg * li);
+                atomicAdd(gLI + ol + t, c * li + reg * r);
+            }
+        }
+        if (lane == 0) {
+            tU[u] = stamp; tI[i] = stamp; tL[l] = stamp;
+            if (PAIRWISE) tI[j] = stamp;
+        }
+    }
+    if (lane == 0 && loss) atomicAdd(loss, loss_acc);
+}
+
+// ---------------------------------------------------------------------------------------------
+// TransRec (TransRec.py:66-91).  v_* = ((p + g) + r) - q_*, x_* = b_* - |v_*|^2, c = dl/dx;
+//   dx/d{p, g, r} = -2 v,  dx/dq = 2 v,  dx/db = 1
+//   pairwise   x = x_i - x_j, reg * l2_loss(p, r, q_j, q_i, b_i, b_j, g)
+//   pointwise  x = x_i,       reg * l2_loss(p, r, q_i, b_i, g)
+// g is one [1, d] variable, so its reg term enters once per batch.  work: gridDim.x partial sums of g's gradient
+// ([gridDim.x, D]) and, after kTransRecCtas * D floats, the CTA completion counter (0 on entry, 0 on exit).
+// ---------------------------------------------------------------------------------------------
+template <bool PAIRWISE>
+__global__ void __launch_bounds__(256)
+transrec_grad_kernel(const float* __restrict__ P, const float* __restrict__ Q, const float* __restrict__ B,
+                     const float* __restrict__ G, int D, const int32_t* __restrict__ users,
+                     const int32_t* __restrict__ recent, const int32_t* __restrict__ items, const void* __restrict__ third,
+                     int64_t batch, int loss_kind, float reg, float inv_b, float* __restrict__ gP, float* __restrict__ gQ,
+                     float* __restrict__ gB, float* __restrict__ gG, int32_t* __restrict__ tP, int32_t* __restrict__ tQ,
+                     int32_t* __restrict__ tB, int32_t stamp, float* __restrict__ work, float* __restrict__ loss) {
+    __shared__ float s_g[kSeqWarps][kSeqMaxDim];
+    __shared__ bool s_last;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float dg[kSeqPerLane];
+#pragma unroll
+    for (int c = 0; c < kSeqPerLane; ++c) dg[c] = 0.0f;
+    float loss_acc = 0.0f;
+    for (int64_t b = blockIdx.x * kSeqWarps + warp; b < batch; b += (int64_t)gridDim.x * kSeqWarps) {
+        const int u = users[b], l = recent[b], i = items[b];
+        const int j = PAIRWISE ? static_cast<const int32_t*>(third)[b] : 0;
+        const size_t ou = (size_t)u * D, ol = (size_t)l * D, oi = (size_t)i * D, oj = (size_t)j * D;
+        float di = 0.f, dj = 0.f, sq = 0.f;
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) {
+            const int t = lane + c * kWarp;
+            if (t < D) {
+                const float p = P[ou + t], r = Q[ol + t], qi = Q[oi + t];
+                const float x = (p + G[t]) + r;          // user + tile(global) + recent (TransRec.py:75-76)
+                const float vi = x - qi;
+                di = fmaf(vi, vi, di);
+                sq += p * p + r * r + qi * qi;
+                if (PAIRWISE) {
+                    const float qj = Q[oj + t], vj = x - qj;
+                    dj = fmaf(vj, vj, dj);
+                    sq += qj * qj;
+                }
+            }
+        }
+        const float bi = B[i], bj = PAIRWISE ? B[j] : 0.0f;
+        const float xi = bi - warp_sum(di);
+        float lo, c;
+        if (PAIRWISE) pairwise_loss_grad(loss_kind, xi - (bj - warp_sum(dj)), lo, c);
+        else pointwise_loss_grad(loss_kind, xi, static_cast<const float*>(third)[b], inv_b, lo, c);
+        if (reg != 0.0f) lo += reg * 0.5f * (warp_sum(sq) + bi * bi + bj * bj);
+        loss_acc += lo;
+        const float c2 = 2.0f * c;
+#pragma unroll
+        for (int k = 0; k < kSeqPerLane; ++k) {
+            const int t = lane + k * kWarp;
+            if (t < D) {
+                const float p = P[ou + t], r = Q[ol + t], qi = Q[oi + t];
+                const float x = (p + G[t]) + r;
+                const float vi = x - qi;
+                float e;                                 // dl/d(p + g + r) without the reg terms
+                if (PAIRWISE) {
+                    const float qj = Q[oj + t], vj = x - qj;
+                    e = -c2 * (vi - vj);
+                    atomicAdd(gQ + oj + t, -c2 * vj + reg * qj);
+                } else {
+                    e = -c2 * vi;
+                }
+                atomicAdd(gP + ou + t, e + reg * p);
+                atomicAdd(gQ + ol + t, e + reg * r);
+                atomicAdd(gQ + oi + t, c2 * vi + reg * qi);
+                dg[k] += e;
+            }
+        }
+        if (lane == 0) {
+            atomicAdd(gB + i, c + reg * bi);
+            tP[u] = stamp; tQ[l] = stamp; tQ[i] = stamp; tB[i] = stamp;
+            if (PAIRWISE) {
+                atomicAdd(gB + j, -c + reg * bj);
+                tQ[j] = stamp; tB[j] = stamp;
+            }
+        }
+    }
+    if (lane == 0 && loss) atomicAdd(loss, loss_acc);
+
+    // g's gradient: this CTA's warps in warp order -> work[blockIdx.x]; the last CTA sums the CTAs in CTA order
+#pragma unroll
+    for (int k = 0; k < kSeqPerLane; ++k) {
+        const int t = lane + k * kWarp;
+        if (t < D) s_g[warp][t] = dg[k];
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < D; t += blockDim.x) {
+        float s = 0.0f;
+#pragma unroll
+        for (int w = 0; w < kSeqWarps; ++w) s += s_g[w][t];
+        work[(size_t)blockIdx.x * D + t] = s;
+    }
+    __threadfence();
+    __syncthreads();
+    unsigned* done = reinterpret_cast<unsigned*>(work + (size_t)kTransRecCtas * D);
+    if (threadIdx.x == 0) s_last = atomicAdd(done, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    for (int t = threadIdx.x; t < D; t += blockDim.x) {
+        float s = 0.0f;
+        for (unsigned k = 0; k < gridDim.x; ++k) s += __ldcg(work + (size_t)k * D + t);
+        gG[t] += s + reg * G[t];
+    }
+    if (warp == 0 && reg != 0.0f && loss) {
+        float sq = 0.0f;
+        for (int t = lane; t < D; t += kWarp) sq += G[t] * G[t];
+        sq = warp_sum(sq);
+        if (lane == 0) atomicAdd(loss, reg * 0.5f * sq);
+    }
+    if (threadIdx.x == 0) *done = 0u;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Scores of every item for kScoreRows (user, recent item) rows per CTA, one item per thread; the rows' query vectors
+// sit in shared memory.  grid = (row groups, item tiles of 256).
+// ---------------------------------------------------------------------------------------------
+// FPMC.predict (FPMC.py:140-165): out[r, j] = <UI_u, IU_j> + <IL_j, LI_l>
+__global__ void __launch_bounds__(256)
+fpmc_scores_kernel(const float* __restrict__ UI, const float* __restrict__ IU, const float* __restrict__ IL,
+                   const float* __restrict__ LI, int D, int32_t num_items, const int32_t* __restrict__ users,
+                   const int32_t* __restrict__ recent, int64_t rows, float* __restrict__ out) {
+    __shared__ float s_u[kScoreRows][kSeqMaxDim], s_l[kScoreRows][kSeqMaxDim];
+    const int64_t r0 = (int64_t)blockIdx.x * kScoreRows;
+    const int nr = (rows - r0 < kScoreRows) ? (int)(rows - r0) : kScoreRows;
+    for (int e = threadIdx.x; e < kScoreRows * D; e += blockDim.x) {
+        const int r = e / D, k = e - r * D;
+        const bool live = r < nr;
+        s_u[r][k] = live ? UI[(size_t)users[r0 + r] * D + k] : 0.0f;
+        s_l[r][k] = live ? LI[(size_t)recent[r0 + r] * D + k] : 0.0f;
+    }
+    __syncthreads();
+    const int64_t j = (int64_t)blockIdx.y * blockDim.x + threadIdx.x;
+    if (j >= num_items) return;
+    const float* __restrict__ iu = IU + (size_t)j * D;
+    const float* __restrict__ il = IL + (size_t)j * D;
+    float acc[kScoreRows];
+#pragma unroll
+    for (int r = 0; r < kScoreRows; ++r) acc[r] = 0.0f;
+    for (int k = 0; k < D; ++k) {
+        const float a = __ldg(iu + k), c = __ldg(il + k);
+#pragma unroll
+        for (int r = 0; r < kScoreRows; ++r) acc[r] = fmaf(c, s_l[r][k], fmaf(s_u[r][k], a, acc[r]));
+    }
+#pragma unroll
+    for (int r = 0; r < kScoreRows; ++r)
+        if (r < nr) out[(size_t)(r0 + r) * num_items + j] = acc[r];
+}
+
+// TransRec's prediction graph (TransRec.py:102-107): out[r, j] = b_j - sqrt(sum_k (x_k - Q_jk)^2), x = (P_u + g) + Q_l.
+// The squared distance is summed from the differences themselves (no |x|^2 - 2 x.q + |q|^2 expansion, which cancels
+// when x is close to q), so x == Q_j gives exactly b_j.
+__global__ void __launch_bounds__(256)
+transrec_scores_kernel(const float* __restrict__ P, const float* __restrict__ Q, const float* __restrict__ B,
+                       const float* __restrict__ G, int D, int32_t num_items, const int32_t* __restrict__ users,
+                       const int32_t* __restrict__ recent, int64_t rows, float* __restrict__ out) {
+    __shared__ float s_x[kScoreRows][kSeqMaxDim];
+    const int64_t r0 = (int64_t)blockIdx.x * kScoreRows;
+    const int nr = (rows - r0 < kScoreRows) ? (int)(rows - r0) : kScoreRows;
+    for (int e = threadIdx.x; e < kScoreRows * D; e += blockDim.x) {
+        const int r = e / D, k = e - r * D;
+        s_x[r][k] = r < nr ? (P[(size_t)users[r0 + r] * D + k] + G[k]) + Q[(size_t)recent[r0 + r] * D + k] : 0.0f;
+    }
+    __syncthreads();
+    const int64_t j = (int64_t)blockIdx.y * blockDim.x + threadIdx.x;
+    if (j >= num_items) return;
+    const float* __restrict__ q = Q + (size_t)j * D;
+    float acc[kScoreRows];
+#pragma unroll
+    for (int r = 0; r < kScoreRows; ++r) acc[r] = 0.0f;
+    for (int k = 0; k < D; ++k) {
+        const float a = __ldg(q + k);
+#pragma unroll
+        for (int r = 0; r < kScoreRows; ++r) {
+            const float v = s_x[r][k] - a;
+            acc[r] = fmaf(v, v, acc[r]);
+        }
+    }
+    const float bj = __ldg(B + j);
+#pragma unroll
+    for (int r = 0; r < kScoreRows; ++r)
+        if (r < nr) out[(size_t)(r0 + r) * num_items + j] = bj - sqrtf(acc[r]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// argument checks shared by the entry points (all of them before any CUDA call: a rejected call writes nothing)
+// ---------------------------------------------------------------------------------------------
+static int seq_check(int32_t dim, int32_t pairwise, int32_t loss_kind, int64_t batch) {
+    NRC_REQUIRE(dim >= 1 && dim <= kSeqMaxDim, NRC_E_LIMIT, "dim %d outside [1, %d]", dim, kSeqMaxDim);
+    // learner.py:27-28 / 39-40
+    if (pairwise)
+        NRC_REQUIRE(loss_kind == NRC_LOSS_BPR || loss_kind == NRC_LOSS_HINGE || loss_kind == NRC_LOSS_SQUARE, NRC_E_VALUE,
+                    "please choose a suitable loss function");
+    else
+        NRC_REQUIRE(loss_kind == NRC_LOSS_CROSS_ENTROPY || loss_kind == NRC_LOSS_SQUARE, NRC_E_VALUE,
+                    "please choose a suitable loss function");
+    NRC_REQUIRE(batch >= 0, NRC_E_VALUE, "batch >= 0 required");
+    return NRC_OK;
+}
+
+static int seq_check_epoch(int32_t dim, int32_t pairwise, int32_t loss_kind, int64_t n, int32_t batch_size,
+                           int32_t opt_kind, const float* lr_t_host, const float* hyper_host) {
+    const int rc = seq_check(dim, pairwise, loss_kind, n);
+    if (rc) return rc;
+    NRC_REQUIRE(batch_size > 0, NRC_E_VALUE, "batch_size should be a positive integeral value");
+    // learner.py:14-15
+    NRC_REQUIRE(opt_kind >= NRC_OPT_GD && opt_kind <= NRC_OPT_MOMENTUM, NRC_E_VALUE, "please select a suitable optimizer");
+    NRC_REQUIRE(lr_t_host && hyper_host, NRC_E_VALUE, "lr_t_host and hyper_host are required");
+    return NRC_OK;
+}
+
+}  // namespace nrc
+
+using namespace nrc;
+
+extern "C" int nrc_fpmc_grad(const float* ui, const float* iu, const float* il, const float* li, int32_t dim,
+                             const int32_t* users, const int32_t* recent, const int32_t* items, const void* third,
+                             int64_t batch, int32_t pairwise, int32_t loss_kind, float reg, float* grad_ui,
+                             float* grad_iu, float* grad_il, float* grad_li, int32_t* touched_user,
+                             int32_t* touched_item, int32_t* touched_recent, int32_t stamp, float* loss, void* stream) {
+    const int rc = seq_check(dim, pairwise, loss_kind, batch);
+    if (rc) return rc;
+    if (batch == 0) return NRC_OK;
+    const unsigned grid = seq_grad_grid(batch, (int64_t)sm_count() * 8);
+    const float inv_b = 1.0f / (float)batch;
+    if (pairwise)
+        fpmc_grad_kernel<true><<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, li, dim, users, recent, items, third, batch,
+                                                                     loss_kind, reg, inv_b, grad_ui, grad_iu, grad_il,
+                                                                     grad_li, touched_user, touched_item, touched_recent,
+                                                                     stamp, loss);
+    else
+        fpmc_grad_kernel<false><<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, li, dim, users, recent, items, third, batch,
+                                                                      loss_kind, reg, inv_b, grad_ui, grad_iu, grad_il,
+                                                                      grad_li, touched_user, touched_item, touched_recent,
+                                                                      stamp, loss);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+extern "C" int nrc_fpmc_train_epoch(float* ui, float* iu, float* il, float* li, int32_t num_users, int32_t num_items,
+                                    int32_t dim, const int32_t* users, const int32_t* recent, const int32_t* items,
+                                    const void* third, int64_t n, int32_t batch_size, int32_t pairwise, int32_t loss_kind,
+                                    float reg, int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                                    float* grad_ui, float* grad_iu, float* grad_il, float* grad_li,
+                                    int32_t* touched_user, int32_t* touched_item, int32_t* touched_recent,
+                                    float* const* slot0, float* const* slot1, int32_t first_stamp, float* step_loss,
+                                    void* stream) {
+    int rc = seq_check_epoch(dim, pairwise, loss_kind, n, batch_size, opt_kind, lr_t_host, hyper_host);
+    if (rc) return rc;
+    NRC_REQUIRE(slot0 && slot1, NRC_E_VALUE, "slot0 and slot1 must list the four variables' slots");
+    cudaStream_t st = as_stream(stream);
+    const int64_t steps = (n + batch_size - 1) / batch_size;
+    if (steps == 0) return NRC_OK;
+    NRC_CUDA_CHECK(cudaMemsetAsync(step_loss, 0, (size_t)steps * sizeof(float), st));
+    float hyper[4] = {hyper_host[0], hyper_host[1], hyper_host[2], hyper_host[3]};
+    const size_t third_bytes = 4;       // i32 negatives or f32 labels
+    for (int64_t s = 0; s < steps; ++s) {
+        const int64_t off = s * batch_size;
+        const int64_t bs = (n - off < batch_size) ? (n - off) : batch_size;
+        const int32_t stamp = first_stamp + (int32_t)s;
+        rc = nrc_fpmc_grad(ui, iu, il, li, dim, users + off, recent + off, items + off,
+                           static_cast<const char*>(third) + off * third_bytes, bs, pairwise, loss_kind, reg, grad_ui,
+                           grad_iu, grad_il, grad_li, touched_user, touched_item, touched_recent, stamp, step_loss + s,
+                           stream);
+        if (rc) return rc;
+        if (opt_kind == NRC_OPT_ADAM) hyper[0] = lr_t_host[s];
+        OptLaunch L;
+        rc = opt_launch_init(L, opt_kind, hyper);
+        if (rc) return rc;
+        opt_launch_add(L, ui, grad_ui, slot0[0], slot1[0], touched_user, num_users, dim, 0);
+        opt_launch_add(L, iu, grad_iu, slot0[1], slot1[1], touched_item, num_items, dim, 0);
+        opt_launch_add(L, il, grad_il, slot0[2], slot1[2], touched_item, num_items, dim, 0);
+        opt_launch_add(L, li, grad_li, slot0[3], slot1[3], touched_recent, num_items, dim, 0);
+        rc = opt_launch_run(L, stamp, st);
+        if (rc) return rc;
+    }
+    return NRC_OK;
+}
+
+extern "C" int64_t nrc_transrec_work_floats(int32_t dim) {
+    NRC_REQUIRE(dim >= 1 && dim <= kSeqMaxDim, NRC_E_LIMIT, "dim %d outside [1, %d]", dim, kSeqMaxDim);
+    return (int64_t)kTransRecCtas * dim + 1;
+}
+
+extern "C" int nrc_transrec_grad(const float* user_table, const float* item_table, const float* item_bias,
+                                 const float* global, int32_t dim, const int32_t* users, const int32_t* recent,
+                                 const int32_t* items, const void* third, int64_t batch, int32_t pairwise,
+                                 int32_t loss_kind, float reg, float* grad_user, float* grad_item, float* grad_bias,
+                                 float* grad_global, int32_t* touched_user, int32_t* touched_item,
+                                 int32_t* touched_bias, int32_t stamp, float* work, float* loss, void* stream) {
+    const int rc = seq_check(dim, pairwise, loss_kind, batch);
+    if (rc) return rc;
+    NRC_REQUIRE(work, NRC_E_VALUE, "work (nrc_transrec_work_floats(dim) floats) is required");
+    if (batch == 0) return NRC_OK;
+    const unsigned grid = seq_grad_grid(batch, kTransRecCtas);
+    const float inv_b = 1.0f / (float)batch;
+    if (pairwise)
+        transrec_grad_kernel<true><<<grid, 256, 0, as_stream(stream)>>>(
+            user_table, item_table, item_bias, global, dim, users, recent, items, third, batch, loss_kind, reg, inv_b,
+            grad_user, grad_item, grad_bias, grad_global, touched_user, touched_item, touched_bias, stamp, work, loss);
+    else
+        transrec_grad_kernel<false><<<grid, 256, 0, as_stream(stream)>>>(
+            user_table, item_table, item_bias, global, dim, users, recent, items, third, batch, loss_kind, reg, inv_b,
+            grad_user, grad_item, grad_bias, grad_global, touched_user, touched_item, touched_bias, stamp, work, loss);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+extern "C" int nrc_transrec_train_epoch(float* user_table, float* item_table, float* item_bias, float* global,
+                                        int32_t num_users, int32_t num_items, int32_t dim, const int32_t* users,
+                                        const int32_t* recent, const int32_t* items, const void* third, int64_t n,
+                                        int32_t batch_size, int32_t pairwise, int32_t loss_kind, float reg,
+                                        int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                                        float* grad_user, float* grad_item, float* grad_bias, float* grad_global,
+                                        int32_t* touched_user, int32_t* touched_item, int32_t* touched_bias,
+                                        float* const* slot0, float* const* slot1, int32_t first_stamp, float* work,
+                                        float* step_loss, void* stream) {
+    int rc = seq_check_epoch(dim, pairwise, loss_kind, n, batch_size, opt_kind, lr_t_host, hyper_host);
+    if (rc) return rc;
+    NRC_REQUIRE(slot0 && slot1, NRC_E_VALUE, "slot0 and slot1 must list the four variables' slots");
+    NRC_REQUIRE(work, NRC_E_VALUE, "work (nrc_transrec_work_floats(dim) floats) is required");
+    cudaStream_t st = as_stream(stream);
+    const int64_t steps = (n + batch_size - 1) / batch_size;
+    if (steps == 0) return NRC_OK;
+    NRC_CUDA_CHECK(cudaMemsetAsync(step_loss, 0, (size_t)steps * sizeof(float), st));
+    float hyper[4] = {hyper_host[0], hyper_host[1], hyper_host[2], hyper_host[3]};
+    const size_t third_bytes = 4;       // i32 negatives or f32 labels
+    for (int64_t s = 0; s < steps; ++s) {
+        const int64_t off = s * batch_size;
+        const int64_t bs = (n - off < batch_size) ? (n - off) : batch_size;
+        const int32_t stamp = first_stamp + (int32_t)s;
+        rc = nrc_transrec_grad(user_table, item_table, item_bias, global, dim, users + off, recent + off, items + off,
+                               static_cast<const char*>(third) + off * third_bytes, bs, pairwise, loss_kind, reg,
+                               grad_user, grad_item, grad_bias, grad_global, touched_user, touched_item, touched_bias,
+                               stamp, work, step_loss + s, stream);
+        if (rc) return rc;
+        if (opt_kind == NRC_OPT_ADAM) hyper[0] = lr_t_host[s];
+        OptLaunch L;
+        rc = opt_launch_init(L, opt_kind, hyper);
+        if (rc) return rc;
+        opt_launch_add(L, user_table, grad_user, slot0[0], slot1[0], touched_user, num_users, dim, 0);
+        opt_launch_add(L, item_table, grad_item, slot0[1], slot1[1], touched_item, num_items, dim, 0);
+        opt_launch_add(L, item_bias, grad_bias, slot0[2], slot1[2], touched_bias, num_items, 1, 0);
+        // tf.tile makes g's gradient a dense tensor: the Apply* formulas, every element (TransRec.py:75)
+        opt_launch_add(L, global, grad_global, slot0[3], slot1[3], nullptr, 1, dim, 1);
+        rc = opt_launch_run(L, stamp, st);
+        if (rc) return rc;
+    }
+    return NRC_OK;
+}
+
+static unsigned score_item_tiles(int32_t num_items) { return (unsigned)((num_items + 255) / 256); }
+
+extern "C" int nrc_fpmc_scores(const float* ui, const float* iu, const float* il, const float* li, int32_t num_items,
+                               int32_t dim, const int32_t* users, const int32_t* recent, int64_t rows, float* out,
+                               void* stream) {
+    NRC_REQUIRE(dim >= 1 && dim <= kSeqMaxDim, NRC_E_LIMIT, "dim %d outside [1, %d]", dim, kSeqMaxDim);
+    NRC_REQUIRE(num_items > 0 && rows >= 0, NRC_E_VALUE, "num_items > 0 and rows >= 0 required");
+    NRC_REQUIRE(score_item_tiles(num_items) <= 65535u, NRC_E_LIMIT, "num_items %d above %d", num_items, 65535 * 256);
+    if (rows == 0) return NRC_OK;
+    const dim3 grid((unsigned)((rows + kScoreRows - 1) / kScoreRows), score_item_tiles(num_items));
+    fpmc_scores_kernel<<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, li, dim, num_items, users, recent, rows, out);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+extern "C" int nrc_transrec_scores(const float* user_table, const float* item_table, const float* item_bias,
+                                   const float* global, int32_t num_items, int32_t dim, const int32_t* users,
+                                   const int32_t* recent, int64_t rows, float* out, void* stream) {
+    NRC_REQUIRE(dim >= 1 && dim <= kSeqMaxDim, NRC_E_LIMIT, "dim %d outside [1, %d]", dim, kSeqMaxDim);
+    NRC_REQUIRE(num_items > 0 && rows >= 0, NRC_E_VALUE, "num_items > 0 and rows >= 0 required");
+    NRC_REQUIRE(score_item_tiles(num_items) <= 65535u, NRC_E_LIMIT, "num_items %d above %d", num_items, 65535 * 256);
+    if (rows == 0) return NRC_OK;
+    const dim3 grid((unsigned)((rows + kScoreRows - 1) / kScoreRows), score_item_tiles(num_items));
+    transrec_scores_kernel<<<grid, 256, 0, as_stream(stream)>>>(user_table, item_table, item_bias, global, dim,
+                                                                 num_items, users, recent, rows, out);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}

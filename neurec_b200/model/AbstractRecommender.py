@@ -1,5 +1,5 @@
-"""AbstractRecommender: the model plug-in base classes (reference model/AbstractRecommender.py:9-80).
-The sequential base is outside the hot path."""
+"""AbstractRecommender: the model plug-in base classes (reference model/AbstractRecommender.py:9-80): the general
+base, the sequential base (models that need the interaction times) and the social base."""
 import os
 import time
 
@@ -41,6 +41,16 @@ class AbstractRecommender(object):
 
     def predict(self, user_ids, items):
         raise NotImplementedError
+
+
+class SeqAbstractRecommender(AbstractRecommender):
+    """AbstractRecommender.py:48-52: a sequential model needs the dataset's time matrix (a UIRT or UIT column
+    format); without it the constructor fails before the evaluator and the logger are built."""
+
+    def __init__(self, dataset, conf):
+        if dataset.time_matrix is None:
+            raise ValueError("Dataset does not contant time infomation!")
+        super(SeqAbstractRecommender, self).__init__(dataset, conf)
 
 
 class SocialAbstractRecommender(AbstractRecommender):

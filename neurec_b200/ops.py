@@ -873,6 +873,105 @@ def sbpr_train_epoch(U, V, B, users, pos, social, neg, suk, batch_size, loss, re
     return steps
 
 
+# ------------------------------------------------------------------------- sequential: FPMC, TransRec
+def _slot_array(slots):
+    """HOST array of four slot pointers (None -> NULL) for the *_train_epoch entry points."""
+    return (ctypes.c_void_p * 4)(*[None if s is None else s.data_ptr() for s in slots])
+
+
+def _epoch_prologue(users, batch_size, lr_t, hyper):
+    n = users.numel()
+    steps = (n + batch_size - 1) // batch_size
+    lr_t = np.ascontiguousarray(lr_t, dtype=np.float32)
+    assert lr_t.size >= max(steps, 1)
+    h = np.zeros(4, dtype=np.float32)
+    h[:len(hyper)] = hyper
+    return n, steps, lr_t, h
+
+
+def fpmc_grad(UI, IU, IL, LI, users, recent, items, third, pairwise, loss, reg, gUI, gIU, gIL, gLI, tU, tI, tL, stamp,
+              loss_out):
+    """Loss + row gradients of one FPMC batch (FPMC.py:61-84); `third` = negatives (i32) or labels (f32)."""
+    check(_lib.load().nrc_fpmc_grad(_p(UI), _p(IU), _p(IL), _p(LI), UI.shape[1], _p(users), _p(recent), _p(items),
+                                    _p(third), users.numel(), 1 if pairwise else 0, LOSS_IDS[loss], float(reg), _p(gUI),
+                                    _p(gIU), _p(gIL), _p(gLI), _p(tU), _p(tI), _p(tL), int(stamp), _p(loss_out),
+                                    _stream()))
+    _count()
+
+
+def fpmc_train_epoch(UI, IU, IL, LI, users, recent, items, third, batch_size, pairwise, loss, reg, opt, lr_t, hyper,
+                     grads, touched, slots0, slots1, first_stamp, step_loss):
+    """One FPMC epoch (FPMC.py:106-131): grads = (gUI, gIU, gIL, gLI), touched = (tU, tI, tL), slots0 / slots1 the
+    four variables' optimizer slots (None where the optimizer keeps none).  Returns the number of steps."""
+    n, steps, lr_t, h = _epoch_prologue(users, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_fpmc_train_epoch(
+        _p(UI), _p(IU), _p(IL), _p(LI), UI.shape[0], IU.shape[0], UI.shape[1], _p(users), _p(recent), _p(items),
+        _p(third), n, int(batch_size), 1 if pairwise else 0, LOSS_IDS[loss], float(reg), OPT_IDS[opt],
+        lr_t.ctypes.data, h.ctypes.data, *[_p(g) for g in grads], *[_p(t) for t in touched],
+        ctypes.cast(s0, ctypes.c_void_p), ctypes.cast(s1, ctypes.c_void_p),
+        int(first_stamp), _p(step_loss), _stream()))
+    _count(2 * steps)
+    return steps
+
+
+def fpmc_scores(UI, IU, IL, LI, users, recent):
+    """FPMC.predict(users, None) on the device: f32 [len(users), num_items] for rows (users[r], recent[r])."""
+    for t, name in ((UI, "UI"), (IU, "IU"), (IL, "IL"), (LI, "LI")):
+        _req(t, torch.float32, name)
+    _req(users, torch.int32, "users"); _req(recent, torch.int32, "recent")
+    out = torch.empty((users.numel(), IU.shape[0]), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_fpmc_scores(_p(UI), _p(IU), _p(IL), _p(LI), IU.shape[0], UI.shape[1], _p(users), _p(recent),
+                                      users.numel(), _p(out), _stream()))
+    _count()
+    return out
+
+
+def transrec_work(dim, device="cuda"):
+    """Zero-filled scratch of the TransRec gradient (g's per-CTA partial sums and a completion counter)."""
+    n = _lib.load().nrc_transrec_work_floats(int(dim))
+    check(int(n) if n < 0 else 0)
+    return torch.zeros(int(n), dtype=torch.float32, device=device)
+
+
+def transrec_grad(P, Q, B, G, users, recent, items, third, pairwise, loss, reg, gP, gQ, gB, gG, tP, tQ, tB, stamp, work,
+                  loss_out):
+    """Loss + gradients of one TransRec batch (TransRec.py:66-91); gG is g's dense gradient f32 [d]."""
+    check(_lib.load().nrc_transrec_grad(_p(P), _p(Q), _p(B), _p(G), P.shape[1], _p(users), _p(recent), _p(items),
+                                        _p(third), users.numel(), 1 if pairwise else 0, LOSS_IDS[loss], float(reg),
+                                        _p(gP), _p(gQ), _p(gB), _p(gG), _p(tP), _p(tQ), _p(tB), int(stamp), _p(work),
+                                        _p(loss_out), _stream()))
+    _count()
+
+
+def transrec_train_epoch(P, Q, B, G, users, recent, items, third, batch_size, pairwise, loss, reg, opt, lr_t, hyper,
+                         grads, touched, slots0, slots1, first_stamp, work, step_loss):
+    """One TransRec epoch (TransRec.py:119-141): grads = (gP, gQ, gB, gG), touched = (tP, tQ, tB), slots in the order
+    P, Q, b, g.  Returns the number of steps."""
+    n, steps, lr_t, h = _epoch_prologue(users, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_transrec_train_epoch(
+        _p(P), _p(Q), _p(B), _p(G), P.shape[0], Q.shape[0], P.shape[1], _p(users), _p(recent), _p(items), _p(third), n,
+        int(batch_size), 1 if pairwise else 0, LOSS_IDS[loss], float(reg), OPT_IDS[opt], lr_t.ctypes.data,
+        h.ctypes.data, *[_p(g) for g in grads], *[_p(t) for t in touched],
+        ctypes.cast(s0, ctypes.c_void_p), ctypes.cast(s1, ctypes.c_void_p),
+        int(first_stamp), _p(work), _p(step_loss), _stream()))
+    _count(2 * steps)
+    return steps
+
+
+def transrec_scores(P, Q, B, G, users, recent):
+    """TransRec's prediction graph on the device: f32 [len(users), num_items], b_j - |(P_u + g) + Q_l - Q_j|."""
+    for t, name in ((P, "P"), (Q, "Q"), (B, "B"), (G, "G")):
+        _req(t, torch.float32, name)
+    _req(users, torch.int32, "users"); _req(recent, torch.int32, "recent")
+    out = torch.empty((users.numel(), Q.shape[0]), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_transrec_scores(_p(P), _p(Q), _p(B), _p(G), Q.shape[0], P.shape[1], _p(users), _p(recent),
+                                          users.numel(), _p(out), _stream()))
+    _count()
+    return out
+
+
 def csr_from_coo(rows, cols, num_rows, num_cols):
     """Interactions -> (indptr i64 [num_rows + 1], indices i32 [distinct]) with ascending duplicate-free rows
     (Dataset.to_csr_matrix + csr_to_user_dict, dataset.py:288-296, tool.py:56-65).  ValueError on ids out of range."""
