@@ -866,7 +866,7 @@ int nrc_wrmf_half_step(const float* fixed, int32_t num_fixed, const int64_t* ind
                        float* work, int32_t* not_spd, void* stream);
 
 /* ======================================================================================
- * Sequential recommenders: FPMC and TransRec (model/sequential_recommender/), high_order = 1
+ * Sequential recommenders over one recent item: FPMC and TransRec (model/sequential_recommender/), high_order = 1
  * ==================================================================================== */
 
 /* Shared conventions.  One batch is (users, recent, items, third) i32 [batch] each, with `third` the negatives (i32,
@@ -945,6 +945,83 @@ int nrc_transrec_train_epoch(float* user_table, float* item_table, float* item_b
 int nrc_transrec_scores(const float* user_table, const float* item_table, const float* item_bias,
                         const float* global, int32_t num_items, int32_t dim, const int32_t* users,
                         const int32_t* recent, int64_t rows, float* out, void* stream);
+
+/* ======================================================================================
+ * Sequential recommenders over a window of recent items: HRM and NPE (model/sequential_recommender/), pointwise
+ * ==================================================================================== */
+
+/* Shared conventions.  One batch is users, items i32 [batch], labels f32 [batch] and recent i32 [batch, window]: each
+ * sample's window of the user's previous items, oldest first -- the layout of TimeOrderPointwiseSampler(high_order =
+ * window) (data/sampler.py:42-68, 216-294).  The loss is learner.pointwise_loss (cross_entropy: the batch mean, square:
+ * the batch sum); the batch loss is ADDED into *loss; row gradients are ADDED into dense accumulators and every row
+ * that receives one gets `stamp` in its touched array, as for FPMC.  l2_loss counts every gathered row, window rows
+ * included, so an id repeated in a window gets reg * row once per occurrence.  NRC_E_LIMIT when dim is outside
+ * [1, 256] or window outside [1, 64]; NRC_E_VALUE with "please choose a suitable loss function" for a loss other than
+ * cross_entropy / square.  A rejected call writes nothing.  The *_train_epoch entry points take slot0 / slot1, lr_t_host,
+ * hyper_host, step_loss and the stamps as nrc_fpmc_train_epoch, with the slot arrays listing the model's variables in
+ * the order given below.
+ *
+ * Predict: the window of user u is train_dict[u][len - window:] as Python evaluates it, so a user with len < window
+ * train items has the shorter window seq[max(0, 2 len - window):].  The query entry points read it from a per-user
+ * table recent i32 [num_users, window] (row u padded after its first recent_len[u] entries, recent_len[u] >= 1) and
+ * pool over that length; scores are then nrc_mf_scores of the query rows against the item rows. */
+
+/* HRM._create_inference / _create_loss, HRM.py:62-91, variables P [U, d] (user_embeddings), E [I, d]
+ * (item_embeddings; window and target share it):
+ *   s = pool_S(E[w_0], .., E[w_{window-1}]),  h = pool_P(P_u, s),  x = <h, E_i>
+ *   l(z, x) + reg * l2_loss(P_u, E[w], E_i)
+ * Pools are elementwise; session_agg / pre_agg = 1 takes the max, 0 the mean (the conf's "max" and anything else).
+ * Gradients as TF: the mean passes grad / count, the max passes (1 / n) * grad to each of the n inputs equal to the
+ * maximum (ties are split).  At window = 1 this is the reference's concat branch.  touched_user <- users,
+ * touched_item <- window items and items (E). */
+int nrc_hrm_grad(const float* user_table, const float* item_table, int32_t dim, int32_t window,
+                 const int32_t* users, const int32_t* recent, const int32_t* items, const float* labels,
+                 int64_t batch, int32_t pre_agg, int32_t session_agg, int32_t loss_kind, float reg,
+                 float* grad_user, float* grad_item, int32_t* touched_user, int32_t* touched_item,
+                 int32_t stamp, float* loss, void* stream);
+
+/* HRM.train_model's batch loop, HRM.py:104-129: per batch nrc_hrm_grad + one optimizer launch over P and E. */
+int nrc_hrm_train_epoch(float* user_table, float* item_table, int32_t num_users, int32_t num_items,
+                        int32_t dim, int32_t window, const int32_t* users, const int32_t* recent,
+                        const int32_t* items, const float* labels, int64_t n, int32_t batch_size,
+                        int32_t pre_agg, int32_t session_agg, int32_t loss_kind, float reg,
+                        int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                        float* grad_user, float* grad_item, int32_t* touched_user, int32_t* touched_item,
+                        float* const* slot0, float* const* slot1, int32_t first_stamp, float* step_loss,
+                        void* stream);
+
+/* HRM.predict's query, HRM.py:135-163: out f32 [rows, dim], out[r] = h of user users[r] over its table window; the
+ * scores of every item are nrc_mf_scores(out, E). */
+int nrc_hrm_query(const float* user_table, const float* item_table, int32_t dim, int32_t window,
+                  const int32_t* users, int64_t rows, const int32_t* recent, const int32_t* recent_len,
+                  int32_t pre_agg, int32_t session_agg, float* out, void* stream);
+
+/* NPE._create_inference / _create_loss, NPE.py:54-71, variables UI [U, d], IU [I, d], IL [I, d]:
+ *   c = sum_l IL[w_l],  x = sum_k relu(UI_u)_k relu(IU_i)_k + relu(IU_i)_k relu(c)_k
+ *   l(z, x) + reg * l2_loss(UI_u, IU_i, IL[w])
+ * relu's gradient is 0 where its input is <= 0 (TF's ReluGrad).  touched_user <- users (UI), touched_item <- items
+ * (IU), touched_recent <- window items (IL).  The epoch's slot arrays list UI, IU, IL. */
+int nrc_npe_grad(const float* ui, const float* iu, const float* il, int32_t dim, int32_t window,
+                 const int32_t* users, const int32_t* recent, const int32_t* items, const float* labels,
+                 int64_t batch, int32_t loss_kind, float reg, float* grad_ui, float* grad_iu,
+                 float* grad_il, int32_t* touched_user, int32_t* touched_item, int32_t* touched_recent,
+                 int32_t stamp, float* loss, void* stream);
+
+/* NPE.train_model's batch loop, NPE.py:84-108: per batch nrc_npe_grad + one optimizer launch over UI, IU and IL. */
+int nrc_npe_train_epoch(float* ui, float* iu, float* il, int32_t num_users, int32_t num_items, int32_t dim,
+                        int32_t window, const int32_t* users, const int32_t* recent, const int32_t* items,
+                        const float* labels, int64_t n, int32_t batch_size, int32_t loss_kind, float reg,
+                        int32_t opt_kind, const float* lr_t_host, const float* hyper_host, float* grad_ui,
+                        float* grad_iu, float* grad_il, int32_t* touched_user, int32_t* touched_item,
+                        int32_t* touched_recent, float* const* slot0, float* const* slot1,
+                        int32_t first_stamp, float* step_loss, void* stream);
+
+/* NPE.predict's query, NPE.py:114-142: out f32 [rows, dim], out[r] = relu(UI_u) + relu(c) for user users[r] over its
+ * table window, and, when out_items is not NULL, out_items f32 [num_items, dim] = relu(IU).  The scores of every item
+ * are nrc_mf_scores(out, out_items): sum_k relu(IU_j)_k (relu(UI_u)_k + relu(c)_k). */
+int nrc_npe_query(const float* ui, const float* iu, const float* il, int32_t num_items, int32_t dim,
+                  int32_t window, const int32_t* users, int64_t rows, const int32_t* recent,
+                  const int32_t* recent_len, float* out, float* out_items, void* stream);
 
 #ifdef __cplusplus
 }

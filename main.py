@@ -29,8 +29,8 @@ def resolve_model(recommender):
         if importlib.util.find_spec(name) is not None:
             return getattr(importlib.import_module(name), recommender)
     raise ImportError("recommender '%s' is outside the accelerated hot path "
-                      "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, WRMF, SBPR, FPMC, TransRec)"
-                      % recommender)
+                      "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, WRMF, SBPR, FPMC, TransRec, "
+                      "HRM, NPE)" % recommender)
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
-// The sequential recommenders that score with embedding tables: FPMC and TransRec, fed by the time-ordered samplers
-// at high_order = 1 (one recent item per sample).
+// The sequential recommenders that score with embedding tables, fed by the time-ordered samplers: FPMC and TransRec
+// at high_order = 1 (one recent item per sample), HRM and NPE over a window of the L most recent items.
 //
 // Replaces (reference paths):
 //   model/sequential_recommender/FPMC.py:61-84       _create_inference / _create_loss (four tables, pairwise / pointwise)
@@ -8,15 +8,21 @@
 //   model/sequential_recommender/TransRec.py:66-91   _create_inference / _create_loss (squared translation distance)
 //   model/sequential_recommender/TransRec.py:110-147 train_model's batch loop
 //   model/sequential_recommender/TransRec.py:102-107,153-166  prediction graph (Euclidean distance, not squared)
+//   model/sequential_recommender/HRM.py:54-91,104-129  pooled window, pooled user, loss; train_model's batch loop
+//   model/sequential_recommender/NPE.py:54-71,84-108   summed window, relu products, loss; train_model's batch loop
+//   model/sequential_recommender/HRM.py:135-163, NPE.py:114-142  predict (query rows here, scores by nrc_mf_scores)
 //
-// Neither score is the inner product of one user row and one item row, so neither goes through the MF kernels:
+// None of the training scores is the inner product of one user row and one item row, so none goes through the MF
+// kernels:
 //   FPMC       x(u, l, i) = <UI_u, IU_i> + <IL_i, LI_l>
 //   TransRec   x(u, l, i) = b_i - |(P_u + g) + Q_l - Q_i|^2          (training)
 //              s(u, l, j) = b_j - |(P_u + g) + Q_l - Q_j|             (prediction)
-// Both gradient kernels run one warp per sample and add row gradients into dense accumulators with atomics (duplicate
-// ids sum, as TF's IndexedSlices de-duplication does).  TransRec's global vector g enters every sample; its gradient
-// is summed per warp, then per CTA in warp order, then across CTAs in CTA order by the last CTA to finish -- a fixed
-// order for a given batch size, and no atomics onto the same d floats.
+//   HRM        x(u, w, i) = <pool_P(P_u, pool_S(E[w_0..L-1])), E_i>
+//   NPE        x(u, w, i) = <relu(UI_u), relu(IU_i)> + <relu(IU_i), relu(sum_l IL[w_l])>
+// Every gradient kernel runs one warp per sample and adds row gradients into dense accumulators with atomics
+// (duplicate ids sum, as TF's IndexedSlices de-duplication does).  TransRec's global vector g enters every sample; its
+// gradient is summed per warp, then per CTA in warp order, then across CTAs in CTA order by the last CTA to finish --
+// a fixed order for a given batch size, and no atomics onto the same d floats.
 #include "common.cuh"
 #include "learner.cuh"
 #include "optim.cuh"
@@ -28,6 +34,7 @@ constexpr int kSeqPerLane = kSeqMaxDim / kWarp;   // row elements one lane holds
 constexpr int kSeqWarps = 8;                      // warps of a 256-thread CTA
 constexpr int kTransRecCtas = 128;                // TransRec gradient grid cap: work holds one partial g per CTA
 constexpr int kScoreRows = 8;                     // score kernels: (user, recent) rows per CTA
+constexpr int kSeqMaxWindow = 64;                 // HRM / NPE: recent items per sample
 
 static unsigned seq_grad_grid(int64_t batch, int64_t cap) {
     int64_t blocks = (batch + kSeqWarps - 1) / kSeqWarps;
@@ -288,6 +295,234 @@ transrec_scores_kernel(const float* __restrict__ P, const float* __restrict__ Q,
 }
 
 // ---------------------------------------------------------------------------------------------
+// HRM (HRM.py:62-91), pointwise.  recent is i32 [batch, L], oldest first; c = dl/dx;
+//   s = pool_S(E[w_0], ..., E[w_{L-1}]),  h = pool_P(P_u, s),  x = <h, E_i>,
+//   l(z, x) + reg * l2_loss(P_u, E[w], E_i)
+// Both pools are elementwise: max (SMAX / PMAX) or mean.  Backward as TF: the mean passes grad / count
+// (_MeanGrad); the max passes (1 / n) * grad to each of the n inputs equal to the maximum (_MinOrMaxGrad: ties split).
+// The window is gathered twice (forward, backward); a lane keeps only its elements of s, the tie counts and dl/ds.
+// ---------------------------------------------------------------------------------------------
+template <bool SMAX, bool PMAX>
+__global__ void __launch_bounds__(256)
+hrm_grad_kernel(const float* __restrict__ P, const float* __restrict__ E, int D, int L,
+                const int32_t* __restrict__ users, const int32_t* __restrict__ recent, const int32_t* __restrict__ items,
+                const float* __restrict__ labels, int64_t batch, int loss_kind, float reg, float inv_b,
+                float* __restrict__ gP, float* __restrict__ gE, int32_t* __restrict__ tP, int32_t* __restrict__ tE,
+                int32_t stamp, float* __restrict__ loss) {
+    const int lane = threadIdx.x & 31;
+    const int64_t wpb = blockDim.x >> 5;
+    const float fl = (float)L;
+    float loss_acc = 0.0f;
+    for (int64_t b = blockIdx.x * wpb + (threadIdx.x >> 5); b < batch; b += (int64_t)gridDim.x * wpb) {
+        const int u = users[b], i = items[b];
+        const int32_t* __restrict__ w = recent + b * L;
+        const size_t ou = (size_t)u * D, oi = (size_t)i * D;
+        float s[kSeqPerLane], cnt[kSeqPerLane], ds[kSeqPerLane];
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) { s[c] = SMAX ? -INFINITY : 0.0f; cnt[c] = 0.0f; }
+        float sq = 0.0f, x = 0.0f;
+        for (int k = 0; k < L; ++k) {
+            const size_t ow = (size_t)w[k] * D;
+#pragma unroll
+            for (int c = 0; c < kSeqPerLane; ++c) {
+                const int t = lane + c * kWarp;
+                if (t < D) {
+                    const float v = E[ow + t];
+                    sq = fmaf(v, v, sq);
+                    if (SMAX) {
+                        if (v > s[c]) { s[c] = v; cnt[c] = 1.0f; }
+                        else if (v == s[c]) cnt[c] += 1.0f;
+                    } else {
+                        s[c] += v;
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) {
+            const int t = lane + c * kWarp;
+            if (t < D) {
+                if (!SMAX) s[c] = s[c] / fl;
+                const float p = P[ou + t], e = E[oi + t];
+                const float h = PMAX ? fmaxf(p, s[c]) : (p + s[c]) / 2.0f;
+                x = fmaf(h, e, x);
+                sq += p * p + e * e;
+            }
+        }
+        x = warp_sum(x);
+        float lo, g;
+        pointwise_loss_grad(loss_kind, x, labels[b], inv_b, lo, g);
+        if (reg != 0.0f) lo += reg * 0.5f * warp_sum(sq);
+        loss_acc += lo;
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) {
+            const int t = lane + c * kWarp;
+            if (t < D) {
+                const float p = P[ou + t], e = E[oi + t];
+                const float h = PMAX ? fmaxf(p, s[c]) : (p + s[c]) / 2.0f;
+                const float dh = g * e;
+                float dp;
+                if (PMAX) {
+                    const float share = 1.0f / ((p == s[c]) ? 2.0f : 1.0f);
+                    dp = (p == h) ? share * dh : 0.0f;
+                    ds[c] = (s[c] == h) ? share * dh : 0.0f;
+                } else {
+                    dp = dh / 2.0f;
+                    ds[c] = dh / 2.0f;
+                }
+                atomicAdd(gP + ou + t, dp + reg * p);
+                atomicAdd(gE + oi + t, g * h + reg * e);
+            }
+        }
+        for (int k = 0; k < L; ++k) {
+            const int wk = w[k];
+            const size_t ow = (size_t)wk * D;
+#pragma unroll
+            for (int c = 0; c < kSeqPerLane; ++c) {
+                const int t = lane + c * kWarp;
+                if (t < D) {
+                    const float v = E[ow + t];
+                    const float dv = SMAX ? ((v == s[c]) ? (1.0f / cnt[c]) * ds[c] : 0.0f) : ds[c] / fl;
+                    atomicAdd(gE + ow + t, dv + reg * v);
+                }
+            }
+            if (lane == 0) tE[wk] = stamp;
+        }
+        if (lane == 0) { tP[u] = stamp; tE[i] = stamp; }
+    }
+    if (lane == 0 && loss) atomicAdd(loss, loss_acc);
+}
+
+// ---------------------------------------------------------------------------------------------
+// NPE (NPE.py:54-71), pointwise.  recent is i32 [batch, L]; c = dl/dx;
+//   ctx = sum_l IL[w_l] (in window order),  x = sum_k relu(UI_u)_k relu(IU_i)_k + relu(IU_i)_k relu(ctx)_k,
+//   l(z, x) + reg * l2_loss(UI_u, IU_i, IL[w])
+// relu's gradient is TF's ReluGrad: zero where the input is <= 0.
+// ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+npe_grad_kernel(const float* __restrict__ UI, const float* __restrict__ IU, const float* __restrict__ IL, int D, int L,
+                const int32_t* __restrict__ users, const int32_t* __restrict__ recent, const int32_t* __restrict__ items,
+                const float* __restrict__ labels, int64_t batch, int loss_kind, float reg, float inv_b,
+                float* __restrict__ gUI, float* __restrict__ gIU, float* __restrict__ gIL, int32_t* __restrict__ tU,
+                int32_t* __restrict__ tI, int32_t* __restrict__ tL, int32_t stamp, float* __restrict__ loss) {
+    const int lane = threadIdx.x & 31;
+    const int64_t wpb = blockDim.x >> 5;
+    float loss_acc = 0.0f;
+    for (int64_t b = blockIdx.x * wpb + (threadIdx.x >> 5); b < batch; b += (int64_t)gridDim.x * wpb) {
+        const int u = users[b], i = items[b];
+        const int32_t* __restrict__ w = recent + b * L;
+        const size_t ou = (size_t)u * D, oi = (size_t)i * D;
+        float ctx[kSeqPerLane];
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) ctx[c] = 0.0f;
+        float sq = 0.0f, x = 0.0f;
+        for (int k = 0; k < L; ++k) {
+            const size_t ow = (size_t)w[k] * D;
+#pragma unroll
+            for (int c = 0; c < kSeqPerLane; ++c) {
+                const int t = lane + c * kWarp;
+                if (t < D) {
+                    const float v = IL[ow + t];
+                    ctx[c] += v;
+                    sq = fmaf(v, v, sq);
+                }
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) {
+            const int t = lane + c * kWarp;
+            if (t < D) {
+                const float a = UI[ou + t], q = IU[oi + t];
+                const float ra = fmaxf(a, 0.0f), rq = fmaxf(q, 0.0f), rc = fmaxf(ctx[c], 0.0f);
+                x += ra * rq + rq * rc;
+                sq += a * a + q * q;
+            }
+        }
+        x = warp_sum(x);
+        float lo, g;
+        pointwise_loss_grad(loss_kind, x, labels[b], inv_b, lo, g);
+        if (reg != 0.0f) lo += reg * 0.5f * warp_sum(sq);
+        loss_acc += lo;
+#pragma unroll
+        for (int c = 0; c < kSeqPerLane; ++c) {
+            const int t = lane + c * kWarp;
+            if (t < D) {
+                const float a = UI[ou + t], q = IU[oi + t];
+                const float ra = fmaxf(a, 0.0f), rq = fmaxf(q, 0.0f), rc = fmaxf(ctx[c], 0.0f);
+                atomicAdd(gUI + ou + t, (a > 0.0f ? g * rq : 0.0f) + reg * a);
+                atomicAdd(gIU + oi + t, (q > 0.0f ? g * ra + g * rc : 0.0f) + reg * q);
+                ctx[c] = ctx[c] > 0.0f ? g * rq : 0.0f;          // dl/dctx from here on
+            }
+        }
+        for (int k = 0; k < L; ++k) {
+            const int wk = w[k];
+            const size_t ow = (size_t)wk * D;
+#pragma unroll
+            for (int c = 0; c < kSeqPerLane; ++c) {
+                const int t = lane + c * kWarp;
+                if (t < D) {
+                    const float v = IL[ow + t];
+                    atomicAdd(gIL + ow + t, ctx[c] + reg * v);
+                }
+            }
+            if (lane == 0) tL[wk] = stamp;
+        }
+        if (lane == 0) { tU[u] = stamp; tI[i] = stamp; }
+    }
+    if (lane == 0 && loss) atomicAdd(loss, loss_acc);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Query rows of HRM / NPE predict, one thread per (row, element).  Row r is user u = users[r] with its window
+// recent[u, 0 .. recent_len[u]) (a per-user table of width L); pools run over the window's actual length.
+// ---------------------------------------------------------------------------------------------
+// HRM: out[r] = h = pool_P(P_u, pool_S(E[window]))
+template <bool SMAX, bool PMAX>
+__global__ void __launch_bounds__(256)
+hrm_query_kernel(const float* __restrict__ P, const float* __restrict__ E, int D, int L,
+                 const int32_t* __restrict__ users, const int32_t* __restrict__ recent,
+                 const int32_t* __restrict__ recent_len, int64_t rows, float* __restrict__ out) {
+    const int64_t total = rows * D;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = e / D;
+        const int t = (int)(e - r * D);
+        const int u = users[r], n = recent_len[u];
+        const int32_t* __restrict__ w = recent + (size_t)u * L;
+        float s = SMAX ? -INFINITY : 0.0f;
+        for (int k = 0; k < n; ++k) {
+            const float v = E[(size_t)w[k] * D + t];
+            s = SMAX ? fmaxf(s, v) : s + v;
+        }
+        if (!SMAX) s = s / (float)n;
+        const float p = P[(size_t)u * D + t];
+        out[e] = PMAX ? fmaxf(p, s) : (p + s) / 2.0f;
+    }
+}
+
+// NPE: out[r] = relu(UI_u) + relu(sum of IL over the window), so that <out[r], relu(IU_j)> is the score
+__global__ void __launch_bounds__(256)
+npe_query_kernel(const float* __restrict__ UI, const float* __restrict__ IL, int D, int L,
+                 const int32_t* __restrict__ users, const int32_t* __restrict__ recent,
+                 const int32_t* __restrict__ recent_len, int64_t rows, float* __restrict__ out) {
+    const int64_t total = rows * D;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = e / D;
+        const int t = (int)(e - r * D);
+        const int u = users[r], n = recent_len[u];
+        const int32_t* __restrict__ w = recent + (size_t)u * L;
+        float ctx = 0.0f;
+        for (int k = 0; k < n; ++k) ctx += IL[(size_t)w[k] * D + t];
+        out[e] = fmaxf(UI[(size_t)u * D + t], 0.0f) + fmaxf(ctx, 0.0f);
+    }
+}
+
+__global__ void __launch_bounds__(256)
+relu_kernel(const float* __restrict__ in, int64_t n, float* __restrict__ out) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x)
+        out[e] = fmaxf(in[e], 0.0f);
+}
+
+// ---------------------------------------------------------------------------------------------
 // argument checks shared by the entry points (all of them before any CUDA call: a rejected call writes nothing)
 // ---------------------------------------------------------------------------------------------
 static int seq_check(int32_t dim, int32_t pairwise, int32_t loss_kind, int64_t batch) {
@@ -311,6 +546,48 @@ static int seq_check_epoch(int32_t dim, int32_t pairwise, int32_t loss_kind, int
     // learner.py:14-15
     NRC_REQUIRE(opt_kind >= NRC_OPT_GD && opt_kind <= NRC_OPT_MOMENTUM, NRC_E_VALUE, "please select a suitable optimizer");
     NRC_REQUIRE(lr_t_host && hyper_host, NRC_E_VALUE, "lr_t_host and hyper_host are required");
+    return NRC_OK;
+}
+
+static int seq_check_window(int32_t window) {
+    NRC_REQUIRE(window >= 1 && window <= kSeqMaxWindow, NRC_E_LIMIT, "window %d outside [1, %d]", window,
+                kSeqMaxWindow);
+    return NRC_OK;
+}
+
+static int seq_check_query(int32_t dim, int32_t window, int64_t rows) {
+    NRC_REQUIRE(dim >= 1 && dim <= kSeqMaxDim, NRC_E_LIMIT, "dim %d outside [1, %d]", dim, kSeqMaxDim);
+    const int rc = seq_check_window(window);
+    if (rc) return rc;
+    NRC_REQUIRE(rows >= 0, NRC_E_VALUE, "rows >= 0 required");
+    return NRC_OK;
+}
+
+// The batch loop of every *_train_epoch: batch s covers samples [s * batch_size, min(n, (s + 1) * batch_size)) and
+// gets stamp first_stamp + s.  grad(off, bs, stamp, loss) runs the model's gradient call for it; add(L) lists the
+// model's variables in the optimizer launch that follows (one launch per batch).
+template <class Grad, class Add>
+static int seq_epoch_loop(int64_t n, int32_t batch_size, int32_t opt_kind, const float* lr_t_host,
+                          const float* hyper_host, int32_t first_stamp, float* step_loss, cudaStream_t st, Grad grad,
+                          Add add) {
+    const int64_t steps = (n + batch_size - 1) / batch_size;
+    if (steps == 0) return NRC_OK;
+    NRC_CUDA_CHECK(cudaMemsetAsync(step_loss, 0, (size_t)steps * sizeof(float), st));
+    float hyper[4] = {hyper_host[0], hyper_host[1], hyper_host[2], hyper_host[3]};
+    for (int64_t s = 0; s < steps; ++s) {
+        const int64_t off = s * batch_size;
+        const int64_t bs = (n - off < batch_size) ? (n - off) : batch_size;
+        const int32_t stamp = first_stamp + (int32_t)s;
+        int rc = grad(off, bs, stamp, step_loss + s);
+        if (rc) return rc;
+        if (opt_kind == NRC_OPT_ADAM) hyper[0] = lr_t_host[s];
+        OptLaunch L;
+        rc = opt_launch_init(L, opt_kind, hyper);
+        if (rc) return rc;
+        add(L);
+        rc = opt_launch_run(L, stamp, st);
+        if (rc) return rc;
+    }
     return NRC_OK;
 }
 
@@ -353,33 +630,21 @@ extern "C" int nrc_fpmc_train_epoch(float* ui, float* iu, float* il, float* li, 
     int rc = seq_check_epoch(dim, pairwise, loss_kind, n, batch_size, opt_kind, lr_t_host, hyper_host);
     if (rc) return rc;
     NRC_REQUIRE(slot0 && slot1, NRC_E_VALUE, "slot0 and slot1 must list the four variables' slots");
-    cudaStream_t st = as_stream(stream);
-    const int64_t steps = (n + batch_size - 1) / batch_size;
-    if (steps == 0) return NRC_OK;
-    NRC_CUDA_CHECK(cudaMemsetAsync(step_loss, 0, (size_t)steps * sizeof(float), st));
-    float hyper[4] = {hyper_host[0], hyper_host[1], hyper_host[2], hyper_host[3]};
     const size_t third_bytes = 4;       // i32 negatives or f32 labels
-    for (int64_t s = 0; s < steps; ++s) {
-        const int64_t off = s * batch_size;
-        const int64_t bs = (n - off < batch_size) ? (n - off) : batch_size;
-        const int32_t stamp = first_stamp + (int32_t)s;
-        rc = nrc_fpmc_grad(ui, iu, il, li, dim, users + off, recent + off, items + off,
-                           static_cast<const char*>(third) + off * third_bytes, bs, pairwise, loss_kind, reg, grad_ui,
-                           grad_iu, grad_il, grad_li, touched_user, touched_item, touched_recent, stamp, step_loss + s,
-                           stream);
-        if (rc) return rc;
-        if (opt_kind == NRC_OPT_ADAM) hyper[0] = lr_t_host[s];
-        OptLaunch L;
-        rc = opt_launch_init(L, opt_kind, hyper);
-        if (rc) return rc;
-        opt_launch_add(L, ui, grad_ui, slot0[0], slot1[0], touched_user, num_users, dim, 0);
-        opt_launch_add(L, iu, grad_iu, slot0[1], slot1[1], touched_item, num_items, dim, 0);
-        opt_launch_add(L, il, grad_il, slot0[2], slot1[2], touched_item, num_items, dim, 0);
-        opt_launch_add(L, li, grad_li, slot0[3], slot1[3], touched_recent, num_items, dim, 0);
-        rc = opt_launch_run(L, stamp, st);
-        if (rc) return rc;
-    }
-    return NRC_OK;
+    return seq_epoch_loop(
+        n, batch_size, opt_kind, lr_t_host, hyper_host, first_stamp, step_loss, as_stream(stream),
+        [&](int64_t off, int64_t bs, int32_t stamp, float* loss) {
+            return nrc_fpmc_grad(ui, iu, il, li, dim, users + off, recent + off, items + off,
+                                 static_cast<const char*>(third) + off * third_bytes, bs, pairwise, loss_kind, reg,
+                                 grad_ui, grad_iu, grad_il, grad_li, touched_user, touched_item, touched_recent, stamp,
+                                 loss, stream);
+        },
+        [&](OptLaunch& L) {
+            opt_launch_add(L, ui, grad_ui, slot0[0], slot1[0], touched_user, num_users, dim, 0);
+            opt_launch_add(L, iu, grad_iu, slot0[1], slot1[1], touched_item, num_items, dim, 0);
+            opt_launch_add(L, il, grad_il, slot0[2], slot1[2], touched_item, num_items, dim, 0);
+            opt_launch_add(L, li, grad_li, slot0[3], slot1[3], touched_recent, num_items, dim, 0);
+        });
 }
 
 extern "C" int64_t nrc_transrec_work_floats(int32_t dim) {
@@ -424,34 +689,22 @@ extern "C" int nrc_transrec_train_epoch(float* user_table, float* item_table, fl
     if (rc) return rc;
     NRC_REQUIRE(slot0 && slot1, NRC_E_VALUE, "slot0 and slot1 must list the four variables' slots");
     NRC_REQUIRE(work, NRC_E_VALUE, "work (nrc_transrec_work_floats(dim) floats) is required");
-    cudaStream_t st = as_stream(stream);
-    const int64_t steps = (n + batch_size - 1) / batch_size;
-    if (steps == 0) return NRC_OK;
-    NRC_CUDA_CHECK(cudaMemsetAsync(step_loss, 0, (size_t)steps * sizeof(float), st));
-    float hyper[4] = {hyper_host[0], hyper_host[1], hyper_host[2], hyper_host[3]};
     const size_t third_bytes = 4;       // i32 negatives or f32 labels
-    for (int64_t s = 0; s < steps; ++s) {
-        const int64_t off = s * batch_size;
-        const int64_t bs = (n - off < batch_size) ? (n - off) : batch_size;
-        const int32_t stamp = first_stamp + (int32_t)s;
-        rc = nrc_transrec_grad(user_table, item_table, item_bias, global, dim, users + off, recent + off, items + off,
-                               static_cast<const char*>(third) + off * third_bytes, bs, pairwise, loss_kind, reg,
-                               grad_user, grad_item, grad_bias, grad_global, touched_user, touched_item, touched_bias,
-                               stamp, work, step_loss + s, stream);
-        if (rc) return rc;
-        if (opt_kind == NRC_OPT_ADAM) hyper[0] = lr_t_host[s];
-        OptLaunch L;
-        rc = opt_launch_init(L, opt_kind, hyper);
-        if (rc) return rc;
-        opt_launch_add(L, user_table, grad_user, slot0[0], slot1[0], touched_user, num_users, dim, 0);
-        opt_launch_add(L, item_table, grad_item, slot0[1], slot1[1], touched_item, num_items, dim, 0);
-        opt_launch_add(L, item_bias, grad_bias, slot0[2], slot1[2], touched_bias, num_items, 1, 0);
-        // tf.tile makes g's gradient a dense tensor: the Apply* formulas, every element (TransRec.py:75)
-        opt_launch_add(L, global, grad_global, slot0[3], slot1[3], nullptr, 1, dim, 1);
-        rc = opt_launch_run(L, stamp, st);
-        if (rc) return rc;
-    }
-    return NRC_OK;
+    return seq_epoch_loop(
+        n, batch_size, opt_kind, lr_t_host, hyper_host, first_stamp, step_loss, as_stream(stream),
+        [&](int64_t off, int64_t bs, int32_t stamp, float* loss) {
+            return nrc_transrec_grad(user_table, item_table, item_bias, global, dim, users + off, recent + off,
+                                     items + off, static_cast<const char*>(third) + off * third_bytes, bs, pairwise,
+                                     loss_kind, reg, grad_user, grad_item, grad_bias, grad_global, touched_user,
+                                     touched_item, touched_bias, stamp, work, loss, stream);
+        },
+        [&](OptLaunch& L) {
+            opt_launch_add(L, user_table, grad_user, slot0[0], slot1[0], touched_user, num_users, dim, 0);
+            opt_launch_add(L, item_table, grad_item, slot0[1], slot1[1], touched_item, num_items, dim, 0);
+            opt_launch_add(L, item_bias, grad_bias, slot0[2], slot1[2], touched_bias, num_items, 1, 0);
+            // tf.tile makes g's gradient a dense tensor: the Apply* formulas, every element (TransRec.py:75)
+            opt_launch_add(L, global, grad_global, slot0[3], slot1[3], nullptr, 1, dim, 1);
+        });
 }
 
 static unsigned score_item_tiles(int32_t num_items) { return (unsigned)((num_items + 255) / 256); }
@@ -480,5 +733,140 @@ extern "C" int nrc_transrec_scores(const float* user_table, const float* item_ta
     transrec_scores_kernel<<<grid, 256, 0, as_stream(stream)>>>(user_table, item_table, item_bias, global, dim,
                                                                  num_items, users, recent, rows, out);
     NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// HRM and NPE entry points
+// ---------------------------------------------------------------------------------------------
+static unsigned elementwise_grid(int64_t total) {
+    int64_t blocks = (total + 255) / 256;
+    const int64_t cap = (int64_t)sm_count() * 16;
+    if (blocks > cap) blocks = cap;
+    return (unsigned)(blocks < 1 ? 1 : blocks);
+}
+
+extern "C" int nrc_hrm_grad(const float* user_table, const float* item_table, int32_t dim, int32_t window,
+                            const int32_t* users, const int32_t* recent, const int32_t* items, const float* labels,
+                            int64_t batch, int32_t pre_agg, int32_t session_agg, int32_t loss_kind, float reg,
+                            float* grad_user, float* grad_item, int32_t* touched_user, int32_t* touched_item,
+                            int32_t stamp, float* loss, void* stream) {
+    int rc = seq_check(dim, 0, loss_kind, batch);
+    if (rc) return rc;
+    rc = seq_check_window(window);
+    if (rc) return rc;
+    if (batch == 0) return NRC_OK;
+    const unsigned grid = seq_grad_grid(batch, (int64_t)sm_count() * 8);
+    auto* kernel = session_agg ? (pre_agg ? hrm_grad_kernel<true, true> : hrm_grad_kernel<true, false>)
+                               : (pre_agg ? hrm_grad_kernel<false, true> : hrm_grad_kernel<false, false>);
+    kernel<<<grid, 256, 0, as_stream(stream)>>>(user_table, item_table, dim, window, users, recent, items, labels,
+                                                batch, loss_kind, reg, 1.0f / (float)batch, grad_user, grad_item,
+                                                touched_user, touched_item, stamp, loss);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+extern "C" int nrc_hrm_train_epoch(float* user_table, float* item_table, int32_t num_users, int32_t num_items,
+                                   int32_t dim, int32_t window, const int32_t* users, const int32_t* recent,
+                                   const int32_t* items, const float* labels, int64_t n, int32_t batch_size,
+                                   int32_t pre_agg, int32_t session_agg, int32_t loss_kind, float reg,
+                                   int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                                   float* grad_user, float* grad_item, int32_t* touched_user, int32_t* touched_item,
+                                   float* const* slot0, float* const* slot1, int32_t first_stamp, float* step_loss,
+                                   void* stream) {
+    int rc = seq_check_window(window);
+    if (rc) return rc;
+    rc = seq_check_epoch(dim, 0, loss_kind, n, batch_size, opt_kind, lr_t_host, hyper_host);
+    if (rc) return rc;
+    NRC_REQUIRE(slot0 && slot1, NRC_E_VALUE, "slot0 and slot1 must list the two variables' slots");
+    return seq_epoch_loop(
+        n, batch_size, opt_kind, lr_t_host, hyper_host, first_stamp, step_loss, as_stream(stream),
+        [&](int64_t off, int64_t bs, int32_t stamp, float* loss) {
+            return nrc_hrm_grad(user_table, item_table, dim, window, users + off, recent + off * window, items + off,
+                                labels + off, bs, pre_agg, session_agg, loss_kind, reg, grad_user, grad_item,
+                                touched_user, touched_item, stamp, loss, stream);
+        },
+        [&](OptLaunch& L) {
+            opt_launch_add(L, user_table, grad_user, slot0[0], slot1[0], touched_user, num_users, dim, 0);
+            opt_launch_add(L, item_table, grad_item, slot0[1], slot1[1], touched_item, num_items, dim, 0);
+        });
+}
+
+extern "C" int nrc_hrm_query(const float* user_table, const float* item_table, int32_t dim, int32_t window,
+                             const int32_t* users, int64_t rows, const int32_t* recent, const int32_t* recent_len,
+                             int32_t pre_agg, int32_t session_agg, float* out, void* stream) {
+    const int rc = seq_check_query(dim, window, rows);
+    if (rc) return rc;
+    if (rows == 0) return NRC_OK;
+    auto* kernel = session_agg ? (pre_agg ? hrm_query_kernel<true, true> : hrm_query_kernel<true, false>)
+                               : (pre_agg ? hrm_query_kernel<false, true> : hrm_query_kernel<false, false>);
+    kernel<<<elementwise_grid(rows * dim), 256, 0, as_stream(stream)>>>(user_table, item_table, dim, window, users,
+                                                                        recent, recent_len, rows, out);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+extern "C" int nrc_npe_grad(const float* ui, const float* iu, const float* il, int32_t dim, int32_t window,
+                            const int32_t* users, const int32_t* recent, const int32_t* items, const float* labels,
+                            int64_t batch, int32_t loss_kind, float reg, float* grad_ui, float* grad_iu,
+                            float* grad_il, int32_t* touched_user, int32_t* touched_item, int32_t* touched_recent,
+                            int32_t stamp, float* loss, void* stream) {
+    int rc = seq_check(dim, 0, loss_kind, batch);
+    if (rc) return rc;
+    rc = seq_check_window(window);
+    if (rc) return rc;
+    if (batch == 0) return NRC_OK;
+    const unsigned grid = seq_grad_grid(batch, (int64_t)sm_count() * 8);
+    npe_grad_kernel<<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, dim, window, users, recent, items, labels, batch,
+                                                         loss_kind, reg, 1.0f / (float)batch, grad_ui, grad_iu,
+                                                         grad_il, touched_user, touched_item, touched_recent, stamp,
+                                                         loss);
+    NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+extern "C" int nrc_npe_train_epoch(float* ui, float* iu, float* il, int32_t num_users, int32_t num_items, int32_t dim,
+                                   int32_t window, const int32_t* users, const int32_t* recent, const int32_t* items,
+                                   const float* labels, int64_t n, int32_t batch_size, int32_t loss_kind, float reg,
+                                   int32_t opt_kind, const float* lr_t_host, const float* hyper_host, float* grad_ui,
+                                   float* grad_iu, float* grad_il, int32_t* touched_user, int32_t* touched_item,
+                                   int32_t* touched_recent, float* const* slot0, float* const* slot1,
+                                   int32_t first_stamp, float* step_loss, void* stream) {
+    int rc = seq_check_window(window);
+    if (rc) return rc;
+    rc = seq_check_epoch(dim, 0, loss_kind, n, batch_size, opt_kind, lr_t_host, hyper_host);
+    if (rc) return rc;
+    NRC_REQUIRE(slot0 && slot1, NRC_E_VALUE, "slot0 and slot1 must list the three variables' slots");
+    return seq_epoch_loop(
+        n, batch_size, opt_kind, lr_t_host, hyper_host, first_stamp, step_loss, as_stream(stream),
+        [&](int64_t off, int64_t bs, int32_t stamp, float* loss) {
+            return nrc_npe_grad(ui, iu, il, dim, window, users + off, recent + off * window, items + off, labels + off,
+                                bs, loss_kind, reg, grad_ui, grad_iu, grad_il, touched_user, touched_item,
+                                touched_recent, stamp, loss, stream);
+        },
+        [&](OptLaunch& L) {
+            opt_launch_add(L, ui, grad_ui, slot0[0], slot1[0], touched_user, num_users, dim, 0);
+            opt_launch_add(L, iu, grad_iu, slot0[1], slot1[1], touched_item, num_items, dim, 0);
+            opt_launch_add(L, il, grad_il, slot0[2], slot1[2], touched_recent, num_items, dim, 0);
+        });
+}
+
+extern "C" int nrc_npe_query(const float* ui, const float* iu, const float* il, int32_t num_items, int32_t dim,
+                             int32_t window, const int32_t* users, int64_t rows, const int32_t* recent,
+                             const int32_t* recent_len, float* out, float* out_items, void* stream) {
+    const int rc = seq_check_query(dim, window, rows);
+    if (rc) return rc;
+    NRC_REQUIRE(num_items > 0 || !out_items, NRC_E_VALUE, "num_items > 0 required with out_items");
+    cudaStream_t st = as_stream(stream);
+    if (rows > 0) {
+        npe_query_kernel<<<elementwise_grid(rows * dim), 256, 0, st>>>(ui, il, dim, window, users, recent, recent_len,
+                                                                       rows, out);
+        NRC_CUDA_CHECK(cudaGetLastError());
+    }
+    if (out_items) {
+        const int64_t total = (int64_t)num_items * dim;
+        relu_kernel<<<elementwise_grid(total), 256, 0, st>>>(iu, total, out_items);
+        NRC_CUDA_CHECK(cudaGetLastError());
+    }
     return NRC_OK;
 }

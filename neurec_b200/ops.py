@@ -875,8 +875,8 @@ def sbpr_train_epoch(U, V, B, users, pos, social, neg, suk, batch_size, loss, re
 
 # ------------------------------------------------------------------------- sequential: FPMC, TransRec
 def _slot_array(slots):
-    """HOST array of four slot pointers (None -> NULL) for the *_train_epoch entry points."""
-    return (ctypes.c_void_p * 4)(*[None if s is None else s.data_ptr() for s in slots])
+    """HOST array of the variables' slot pointers (None -> NULL) for the *_train_epoch entry points."""
+    return (ctypes.c_void_p * len(slots))(*[None if s is None else s.data_ptr() for s in slots])
 
 
 def _epoch_prologue(users, batch_size, lr_t, hyper):
@@ -970,6 +970,89 @@ def transrec_scores(P, Q, B, G, users, recent):
                                           users.numel(), _p(out), _stream()))
     _count()
     return out
+
+
+# ------------------------------------------------------------------------- sequential over a window: HRM, NPE
+def _window(recent):
+    """recent i32 [n, L] (or [n] at L = 1) -> L."""
+    return 1 if recent.dim() == 1 else recent.shape[1]
+
+
+def hrm_grad(P, E, users, recent, items, labels, pre_agg, session_agg, loss, reg, gP, gE, tP, tE, stamp, loss_out):
+    """Loss + row gradients of one HRM batch (HRM.py:62-91); recent i32 [batch, L]; pre_agg / session_agg True = max."""
+    check(_lib.load().nrc_hrm_grad(_p(P), _p(E), P.shape[1], _window(recent), _p(users), _p(recent), _p(items),
+                                   _p(labels), users.numel(), int(bool(pre_agg)), int(bool(session_agg)),
+                                   LOSS_IDS[loss], float(reg), _p(gP), _p(gE), _p(tP), _p(tE), int(stamp),
+                                   _p(loss_out), _stream()))
+    _count()
+
+
+def hrm_train_epoch(P, E, users, recent, items, labels, batch_size, pre_agg, session_agg, loss, reg, opt, lr_t, hyper,
+                    grads, touched, slots0, slots1, first_stamp, step_loss):
+    """One HRM epoch (HRM.py:104-129): grads = (gP, gE), touched = (tP, tE), slots in the order P, E.  Returns the
+    number of steps."""
+    n, steps, lr_t, h = _epoch_prologue(users, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_hrm_train_epoch(
+        _p(P), _p(E), P.shape[0], E.shape[0], P.shape[1], _window(recent), _p(users), _p(recent), _p(items),
+        _p(labels), n, int(batch_size), int(bool(pre_agg)), int(bool(session_agg)), LOSS_IDS[loss], float(reg),
+        OPT_IDS[opt], lr_t.ctypes.data, h.ctypes.data, *[_p(g) for g in grads], *[_p(t) for t in touched],
+        ctypes.cast(s0, ctypes.c_void_p), ctypes.cast(s1, ctypes.c_void_p), int(first_stamp), _p(step_loss),
+        _stream()))
+    _count(2 * steps)
+    return steps
+
+
+def _query_args(users, recent, recent_len):
+    _req(users, torch.int32, "users"); _req(recent, torch.int32, "recent"); _req(recent_len, torch.int32, "recent_len")
+    return _window(recent), _p(users), users.numel(), _p(recent), _p(recent_len)
+
+
+def hrm_scores(P, E, users, recent, recent_len, pre_agg, session_agg):
+    """HRM.predict(users, None) on the device: f32 [len(users), num_items].  recent i32 [num_users, L] / recent_len
+    i32 [num_users] hold every user's predict window; the query rows h go through nrc_mf_scores."""
+    _req(P, torch.float32, "P"); _req(E, torch.float32, "E")
+    q = torch.empty((users.numel(), P.shape[1]), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_hrm_query(_p(P), _p(E), P.shape[1], *_query_args(users, recent, recent_len),
+                                    int(bool(pre_agg)), int(bool(session_agg)), _p(q), _stream()))
+    _count()
+    return mf_scores(q, E, torch.arange(users.numel(), dtype=torch.int32, device=users.device))
+
+
+def npe_scores(UI, IU, IL, users, recent, recent_len):
+    """NPE.predict(users, None) on the device: f32 [len(users), num_items], the query rows relu(UI_u) + relu(c)
+    against relu(IU) through nrc_mf_scores."""
+    for t, name in ((UI, "UI"), (IU, "IU"), (IL, "IL")):
+        _req(t, torch.float32, name)
+    q = torch.empty((users.numel(), UI.shape[1]), dtype=torch.float32, device=users.device)
+    items = torch.empty_like(IU)
+    check(_lib.load().nrc_npe_query(_p(UI), _p(IU), _p(IL), IU.shape[0], UI.shape[1],
+                                    *_query_args(users, recent, recent_len), _p(q), _p(items), _stream()))
+    _count(2)
+    return mf_scores(q, items, torch.arange(users.numel(), dtype=torch.int32, device=users.device))
+
+
+def npe_grad(UI, IU, IL, users, recent, items, labels, loss, reg, gUI, gIU, gIL, tU, tI, tL, stamp, loss_out):
+    """Loss + row gradients of one NPE batch (NPE.py:54-71); recent i32 [batch, L]."""
+    check(_lib.load().nrc_npe_grad(_p(UI), _p(IU), _p(IL), UI.shape[1], _window(recent), _p(users), _p(recent),
+                                   _p(items), _p(labels), users.numel(), LOSS_IDS[loss], float(reg), _p(gUI), _p(gIU),
+                                   _p(gIL), _p(tU), _p(tI), _p(tL), int(stamp), _p(loss_out), _stream()))
+    _count()
+
+
+def npe_train_epoch(UI, IU, IL, users, recent, items, labels, batch_size, loss, reg, opt, lr_t, hyper, grads, touched,
+                    slots0, slots1, first_stamp, step_loss):
+    """One NPE epoch (NPE.py:84-108): grads = (gUI, gIU, gIL), touched = (tU, tI, tL), slots in the order UI, IU, IL.
+    Returns the number of steps."""
+    n, steps, lr_t, h = _epoch_prologue(users, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_npe_train_epoch(
+        _p(UI), _p(IU), _p(IL), UI.shape[0], IU.shape[0], UI.shape[1], _window(recent), _p(users), _p(recent),
+        _p(items), _p(labels), n, int(batch_size), LOSS_IDS[loss], float(reg), OPT_IDS[opt], lr_t.ctypes.data,
+        h.ctypes.data, *[_p(g) for g in grads], *[_p(t) for t in touched], ctypes.cast(s0, ctypes.c_void_p),
+        ctypes.cast(s1, ctypes.c_void_p), int(first_stamp), _p(step_loss), _stream()))
+    _count(2 * steps)
+    return steps
 
 
 def csr_from_coo(rows, cols, num_rows, num_cols):
