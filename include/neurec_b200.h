@@ -1023,6 +1023,26 @@ int nrc_npe_query(const float* ui, const float* iu, const float* il, int32_t num
                   int32_t window, const int32_t* users, int64_t rows, const int32_t* recent,
                   const int32_t* recent_len, float* out, float* out_items, void* stream);
 
+/* Test hook of the sequential kernels (it reports and changes nothing; every route is chosen by the shape).
+ * nrc_seq_last_routes: HOST bookkeeping of the most recent launch of each kernel group, written when a call launches
+ * (a call that returns before launching, for a failed check, an empty batch or no rows, leaves it as it was); one
+ * record per process.  out i32[9 * 7], group k at out[7 * k]; -1 = no such launch yet, or a field the group does not
+ * decide.
+ *   groups: [0] nrc_fpmc_grad, [1] nrc_transrec_grad, [2] nrc_hrm_grad, [3] nrc_npe_grad (each also inside its
+ *   *_train_epoch); [4] nrc_fpmc_scores, [5] nrc_transrec_scores; [6] nrc_hrm_query, [7] the query rows of
+ *   nrc_npe_query; [8] the relu pass of nrc_npe_query over the items (out_items).
+ *   fields of a group:
+ *   +0 1 the pairwise form, 0 the pointwise one (gradient kernels);
+ *   +1 HRM: 1 when the window pool (session_agg) is the max, 0 the mean;
+ *   +2 HRM: 1 when the user pool (pre_agg) is the max, 0 the mean;
+ *   +3 CTAs launched (gridDim.x); score kernels: groups of 8 rows;
+ *   +4 score kernels: item tiles of 256 (gridDim.y);
+ *   +5 1 when the grid was capped, so a warp or thread takes more than one sample or element: FPMC, HRM and NPE
+ *      gradients above 64 * SMs samples, TransRec's above 1024 (128 CTAs), the query and relu passes above
+ *      4096 * SMs elements; else 0;
+ *   +6 the window L (HRM and NPE). */
+int nrc_seq_last_routes(int32_t* out);
+
 #ifdef __cplusplus
 }
 #endif

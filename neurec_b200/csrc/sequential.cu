@@ -43,6 +43,28 @@ static unsigned seq_grad_grid(int64_t batch, int64_t cap) {
     return (unsigned)blocks;
 }
 
+// Host record of what the most recent launch of each kernel group decided, for nrc_seq_last_routes (see the header);
+// -1 = no such launch yet, or a field the group does not decide.  Written just before the launch, so a call that fails
+// its checks or launches nothing leaves it as it was.
+enum SeqKernel { kSeqFpmcGrad, kSeqTransRecGrad, kSeqHrmGrad, kSeqNpeGrad, kSeqFpmcScores, kSeqTransRecScores,
+                 kSeqHrmQuery, kSeqNpeQuery, kSeqNpeRelu, kSeqKernels };
+enum SeqRouteField { kSeqPairwise, kSeqSessionMax, kSeqPreMax, kSeqGridX, kSeqGridY, kSeqCapped, kSeqWindow,
+                     kSeqFields };
+static struct SeqRoutes {
+    int32_t r[kSeqKernels][kSeqFields];
+    SeqRoutes() { for (auto& k : r) for (auto& f : k) f = -1; }
+} g_seq_routes;
+
+static void seq_route(int kernel, int pairwise, int session_max, int pre_max, int64_t grid_x, int64_t grid_y,
+                      int capped, int window) {
+    int32_t* r = g_seq_routes.r[kernel];
+    r[kSeqPairwise] = pairwise; r[kSeqSessionMax] = session_max; r[kSeqPreMax] = pre_max;
+    r[kSeqGridX] = (int32_t)grid_x; r[kSeqGridY] = (int32_t)grid_y; r[kSeqCapped] = capped; r[kSeqWindow] = window;
+}
+
+// 1 when seq_grad_grid capped the grid, so a warp takes more than one sample
+static int seq_grad_capped(int64_t batch, int64_t cap) { return (batch + kSeqWarps - 1) / kSeqWarps > cap ? 1 : 0; }
+
 // ---------------------------------------------------------------------------------------------
 // FPMC (FPMC.py:61-84).  c = dl/dx;
 //   pairwise   x = x_i - x_j, reg * l2_loss(UI_u, IU_i, IL_i, LI_l, IU_j, IL_j)
@@ -603,7 +625,9 @@ extern "C" int nrc_fpmc_grad(const float* ui, const float* iu, const float* il, 
     const int rc = seq_check(dim, pairwise, loss_kind, batch);
     if (rc) return rc;
     if (batch == 0) return NRC_OK;
-    const unsigned grid = seq_grad_grid(batch, (int64_t)sm_count() * 8);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const unsigned grid = seq_grad_grid(batch, cap);
+    seq_route(kSeqFpmcGrad, pairwise ? 1 : 0, -1, -1, grid, -1, seq_grad_capped(batch, cap), -1);
     const float inv_b = 1.0f / (float)batch;
     if (pairwise)
         fpmc_grad_kernel<true><<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, li, dim, users, recent, items, third, batch,
@@ -663,6 +687,7 @@ extern "C" int nrc_transrec_grad(const float* user_table, const float* item_tabl
     NRC_REQUIRE(work, NRC_E_VALUE, "work (nrc_transrec_work_floats(dim) floats) is required");
     if (batch == 0) return NRC_OK;
     const unsigned grid = seq_grad_grid(batch, kTransRecCtas);
+    seq_route(kSeqTransRecGrad, pairwise ? 1 : 0, -1, -1, grid, -1, seq_grad_capped(batch, kTransRecCtas), -1);
     const float inv_b = 1.0f / (float)batch;
     if (pairwise)
         transrec_grad_kernel<true><<<grid, 256, 0, as_stream(stream)>>>(
@@ -717,6 +742,7 @@ extern "C" int nrc_fpmc_scores(const float* ui, const float* iu, const float* il
     NRC_REQUIRE(score_item_tiles(num_items) <= 65535u, NRC_E_LIMIT, "num_items %d above %d", num_items, 65535 * 256);
     if (rows == 0) return NRC_OK;
     const dim3 grid((unsigned)((rows + kScoreRows - 1) / kScoreRows), score_item_tiles(num_items));
+    seq_route(kSeqFpmcScores, -1, -1, -1, grid.x, grid.y, -1, -1);
     fpmc_scores_kernel<<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, li, dim, num_items, users, recent, rows, out);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
@@ -730,6 +756,7 @@ extern "C" int nrc_transrec_scores(const float* user_table, const float* item_ta
     NRC_REQUIRE(score_item_tiles(num_items) <= 65535u, NRC_E_LIMIT, "num_items %d above %d", num_items, 65535 * 256);
     if (rows == 0) return NRC_OK;
     const dim3 grid((unsigned)((rows + kScoreRows - 1) / kScoreRows), score_item_tiles(num_items));
+    seq_route(kSeqTransRecScores, -1, -1, -1, grid.x, grid.y, -1, -1);
     transrec_scores_kernel<<<grid, 256, 0, as_stream(stream)>>>(user_table, item_table, item_bias, global, dim,
                                                                  num_items, users, recent, rows, out);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -746,6 +773,9 @@ static unsigned elementwise_grid(int64_t total) {
     return (unsigned)(blocks < 1 ? 1 : blocks);
 }
 
+// 1 when elementwise_grid capped the grid, so a thread takes more than one element
+static int elementwise_capped(int64_t total) { return (total + 255) / 256 > (int64_t)sm_count() * 16 ? 1 : 0; }
+
 extern "C" int nrc_hrm_grad(const float* user_table, const float* item_table, int32_t dim, int32_t window,
                             const int32_t* users, const int32_t* recent, const int32_t* items, const float* labels,
                             int64_t batch, int32_t pre_agg, int32_t session_agg, int32_t loss_kind, float reg,
@@ -756,7 +786,9 @@ extern "C" int nrc_hrm_grad(const float* user_table, const float* item_table, in
     rc = seq_check_window(window);
     if (rc) return rc;
     if (batch == 0) return NRC_OK;
-    const unsigned grid = seq_grad_grid(batch, (int64_t)sm_count() * 8);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const unsigned grid = seq_grad_grid(batch, cap);
+    seq_route(kSeqHrmGrad, 0, session_agg ? 1 : 0, pre_agg ? 1 : 0, grid, -1, seq_grad_capped(batch, cap), window);
     auto* kernel = session_agg ? (pre_agg ? hrm_grad_kernel<true, true> : hrm_grad_kernel<true, false>)
                                : (pre_agg ? hrm_grad_kernel<false, true> : hrm_grad_kernel<false, false>);
     kernel<<<grid, 256, 0, as_stream(stream)>>>(user_table, item_table, dim, window, users, recent, items, labels,
@@ -800,8 +832,11 @@ extern "C" int nrc_hrm_query(const float* user_table, const float* item_table, i
     if (rows == 0) return NRC_OK;
     auto* kernel = session_agg ? (pre_agg ? hrm_query_kernel<true, true> : hrm_query_kernel<true, false>)
                                : (pre_agg ? hrm_query_kernel<false, true> : hrm_query_kernel<false, false>);
-    kernel<<<elementwise_grid(rows * dim), 256, 0, as_stream(stream)>>>(user_table, item_table, dim, window, users,
-                                                                        recent, recent_len, rows, out);
+    const unsigned grid = elementwise_grid(rows * dim);
+    seq_route(kSeqHrmQuery, -1, session_agg ? 1 : 0, pre_agg ? 1 : 0, grid, -1, elementwise_capped(rows * dim),
+              window);
+    kernel<<<grid, 256, 0, as_stream(stream)>>>(user_table, item_table, dim, window, users, recent, recent_len, rows,
+                                                out);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
 }
@@ -816,7 +851,9 @@ extern "C" int nrc_npe_grad(const float* ui, const float* iu, const float* il, i
     rc = seq_check_window(window);
     if (rc) return rc;
     if (batch == 0) return NRC_OK;
-    const unsigned grid = seq_grad_grid(batch, (int64_t)sm_count() * 8);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const unsigned grid = seq_grad_grid(batch, cap);
+    seq_route(kSeqNpeGrad, 0, -1, -1, grid, -1, seq_grad_capped(batch, cap), window);
     npe_grad_kernel<<<grid, 256, 0, as_stream(stream)>>>(ui, iu, il, dim, window, users, recent, items, labels, batch,
                                                          loss_kind, reg, 1.0f / (float)batch, grad_ui, grad_iu,
                                                          grad_il, touched_user, touched_item, touched_recent, stamp,
@@ -859,14 +896,25 @@ extern "C" int nrc_npe_query(const float* ui, const float* iu, const float* il, 
     NRC_REQUIRE(num_items > 0 || !out_items, NRC_E_VALUE, "num_items > 0 required with out_items");
     cudaStream_t st = as_stream(stream);
     if (rows > 0) {
-        npe_query_kernel<<<elementwise_grid(rows * dim), 256, 0, st>>>(ui, il, dim, window, users, recent, recent_len,
-                                                                       rows, out);
+        const unsigned grid = elementwise_grid(rows * dim);
+        seq_route(kSeqNpeQuery, -1, -1, -1, grid, -1, elementwise_capped(rows * dim), window);
+        npe_query_kernel<<<grid, 256, 0, st>>>(ui, il, dim, window, users, recent, recent_len, rows, out);
         NRC_CUDA_CHECK(cudaGetLastError());
     }
     if (out_items) {
         const int64_t total = (int64_t)num_items * dim;
-        relu_kernel<<<elementwise_grid(total), 256, 0, st>>>(iu, total, out_items);
+        const unsigned grid = elementwise_grid(total);
+        seq_route(kSeqNpeRelu, -1, -1, -1, grid, -1, elementwise_capped(total), -1);
+        relu_kernel<<<grid, 256, 0, st>>>(iu, total, out_items);
         NRC_CUDA_CHECK(cudaGetLastError());
     }
+    return NRC_OK;
+}
+
+// Host bookkeeping of the routes the most recent sequential launches took (see the header); no device work.
+extern "C" int nrc_seq_last_routes(int32_t* out) {
+    NRC_REQUIRE(out != nullptr, NRC_E_VALUE, "out is NULL");
+    for (int k = 0; k < kSeqKernels; ++k)
+        for (int f = 0; f < kSeqFields; ++f) out[k * kSeqFields + f] = g_seq_routes.r[k][f];
     return NRC_OK;
 }

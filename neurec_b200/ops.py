@@ -1055,6 +1055,20 @@ def npe_train_epoch(UI, IU, IL, users, recent, items, labels, batch_size, loss, 
     return steps
 
 
+SEQ_KERNELS = ("fpmc_grad", "transrec_grad", "hrm_grad", "npe_grad", "fpmc_scores", "transrec_scores", "hrm_query",
+               "npe_query", "npe_relu")
+SEQ_ROUTE_FIELDS = ("pairwise", "session_max", "pre_max", "grid_x", "grid_y", "capped", "window")
+
+
+def seq_last_routes():
+    """Routes of the most recent launch of each sequential kernel group (nrc_seq_last_routes) as
+    {kernel: {field: value}}; -1 = no such launch yet or a field the group does not decide."""
+    nf = len(SEQ_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(SEQ_KERNELS) * nf))()
+    check(_lib.load().nrc_seq_last_routes(out))
+    return {k: dict(zip(SEQ_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(SEQ_KERNELS)}
+
+
 def csr_from_coo(rows, cols, num_rows, num_cols):
     """Interactions -> (indptr i64 [num_rows + 1], indices i32 [distinct]) with ascending duplicate-free rows
     (Dataset.to_csr_matrix + csr_to_user_dict, dataset.py:288-296, tool.py:56-65).  ValueError on ids out of range."""
