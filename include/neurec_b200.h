@@ -1023,6 +1023,79 @@ int nrc_npe_query(const float* ui, const float* iu, const float* il, int32_t num
                   int32_t window, const int32_t* users, int64_t rows, const int32_t* recent,
                   const int32_t* recent_len, float* out, float* out_items, void* stream);
 
+/* ======================================================================================
+ * FPMCplus (model/sequential_recommender/FPMCplus.py): attention over a window of recent items, conditioned on the
+ * candidate item, pairwise or pointwise
+ * ==================================================================================== */
+
+/* FPMCplus._attention_mlp / _create_inference / _create_loss, FPMCplus.py:53-119.  Variables UI [U, d], IU, IL, LI
+ * [I, d], W [3d, weight_size] (rows [0, d) for the user, [d, 2d) for the item, [2d, 3d) for the window item), b and h
+ * [weight_size].  For user u, window l_1..l_L and item i:
+ *   e_k = <h, tanh([UI_u, IL_i, LI_{l_k}] W + b)>,  a_k = exp(e_k) / sum_k exp(e_k)   (no max shift)
+ *   x   = <UI_u, IU_i> + <IL_i, sum_k a_k LI_{l_k}>
+ *   pairwise   l(x_i - x_j) + reg_mf * l2_loss(UI_u, IU_i, IL_i, LI_w, IU_j, IL_j) + reg_w * l2_loss(W, h)
+ *   pointwise  l(z, x_i)    + reg_mf * l2_loss(UI_u, IU_i, IL_i, LI_w)              (reg_w is not used)
+ * The batch layout, losses, loss and row-gradient accumulation and touched rules are those of the HRM / NPE section
+ * (recent i32 [batch, window]) with `third` as for FPMC: touched_user <- users (UI), touched_item <- items and
+ * negatives (IU and IL), touched_recent <- window items (LI).  grad_w, grad_b and grad_h are dense gradients: every
+ * sample's factors go to work and are summed over the batch in one fixed order (no atomics onto them), so they are
+ * the same bits on every call with the same inputs.  The reg_w term of the loss counts once per batch.
+ * NRC_E_LIMIT when dim is outside [1, 256], weight_size outside [1, 128], window outside [1, 64] or batch above
+ * 65535 * 32; NRC_E_VALUE for a loss the mode does not define or a NULL table, gradient or work.  A rejected call
+ * writes nothing. */
+
+/* Scratch of nrc_fpmcplus_grad / nrc_fpmcplus_train_epoch in floats, for batches of up to batch_size samples:
+ * completion counters, per-sample factors of the dense gradients and per-chunk partial sums.  Zero-fill it once
+ * before its first use; every call leaves the counters ready for the next (calls that share one work buffer must not
+ * run concurrently).  Negative NRC_E_* when an argument is out of range. */
+int64_t nrc_fpmcplus_work_floats(int32_t dim, int32_t weight_size, int32_t window, int32_t batch_size);
+
+int nrc_fpmcplus_grad(const float* ui, const float* iu, const float* il, const float* li, const float* w,
+                      const float* b, const float* h, int32_t dim, int32_t weight_size, int32_t window,
+                      const int32_t* users, const int32_t* recent, const int32_t* items, const void* third,
+                      int64_t batch, int32_t pairwise, int32_t loss_kind, float reg_mf, float reg_w,
+                      float* grad_ui, float* grad_iu, float* grad_il, float* grad_li, float* grad_w,
+                      float* grad_b, float* grad_h, int32_t* touched_user, int32_t* touched_item,
+                      int32_t* touched_recent, int32_t stamp, float* work, float* loss, void* stream);
+
+/* FPMCplus.train_model's batch loop, FPMCplus.py:141-171: per batch nrc_fpmcplus_grad + one optimizer launch over
+ * UI, IU, IL, LI (IndexedSlices rules) and W, b, h (dense rules).  slot0 / slot1: HOST arrays of the seven variables'
+ * slot pointers in that order; the rest as nrc_fpmc_train_epoch. */
+int nrc_fpmcplus_train_epoch(float* ui, float* iu, float* il, float* li, float* w, float* b, float* h,
+                             int32_t num_users, int32_t num_items, int32_t dim, int32_t weight_size,
+                             int32_t window, const int32_t* users, const int32_t* recent, const int32_t* items,
+                             const void* third, int64_t n, int32_t batch_size, int32_t pairwise, int32_t loss_kind,
+                             float reg_mf, float reg_w, int32_t opt_kind, const float* lr_t_host,
+                             const float* hyper_host, float* grad_ui, float* grad_iu, float* grad_il,
+                             float* grad_li, float* grad_w, float* grad_b, float* grad_h, int32_t* touched_user,
+                             int32_t* touched_item, int32_t* touched_recent, float* const* slot0,
+                             float* const* slot1, int32_t first_stamp, float* work, float* step_loss, void* stream);
+
+/* Scratch of nrc_fpmcplus_scores in floats: the item-side projection IL W_I and the transposed IL and IU
+ * (num_items * (weight_size + 2 dim)), and every row's UI_u W_U + b and window projections LI W_L
+ * (rows * (window + 1) * weight_size).  No initialisation needed. */
+int64_t nrc_fpmcplus_score_work_floats(int32_t num_items, int32_t dim, int32_t weight_size, int32_t window,
+                                       int64_t rows);
+
+/* FPMCplus.predict, FPMCplus.py:177-205: out f32 [rows, num_items], out[r, j] = x(users[r], window, j) over the user's
+ * table window (recent / recent_len as for nrc_hrm_query; a window shorter than `window` takes the softmax over its
+ * actual length).  Where sum_k exp(e_k) overflows, the score is NaN if some exp(e_k) overflowed and
+ * <UI_u, IU_j> otherwise, as the reference's exp / sum gives it. */
+int nrc_fpmcplus_scores(const float* ui, const float* iu, const float* il, const float* li, const float* w,
+                        const float* b, const float* h, int32_t num_items, int32_t dim, int32_t weight_size,
+                        int32_t window, const int32_t* users, int64_t rows, const int32_t* recent,
+                        const int32_t* recent_len, float* work, float* out, void* stream);
+
+/* Test hook of the FPMCplus kernels, as nrc_seq_last_routes: out i32[4 * 6], group k at out[6 * k].
+ *   groups: [0] the per-sample gradient kernel, [1] the dense-gradient reduction (both also inside
+ *   nrc_fpmcplus_train_epoch), [2] the projection pass of nrc_fpmcplus_scores, [3] its pair kernel.
+ *   fields: +0 1 the pairwise form, 0 the pointwise one (gradient groups); +1 gridDim.x (CTAs; the reduction: element
+ *   tiles of 256; the pair kernel: row groups); +2 gridDim.y (the reduction: chunks of 32 samples; the pair kernel:
+ *   item tiles of 256); +3 1 when the grid was capped (the gradient kernel above 64 * SMs samples, the projection
+ *   above 4096 * SMs elements), else 0; +4 the window L; +5 the pair kernel's rows per CTA (at most 8, fewer where
+ *   their window rows would not fit in shared memory). */
+int nrc_fpmcplus_last_routes(int32_t* out);
+
 /* Test hook of the sequential kernels (it reports and changes nothing; every route is chosen by the shape).
  * nrc_seq_last_routes: HOST bookkeeping of the most recent launch of each kernel group, written when a call launches
  * (a call that returns before launching, for a failed check, an empty batch or no rows, leaves it as it was); one

@@ -1,2 +1,2 @@
-"""Sequential recommenders on the time-ordered samplers: FPMC and TransRec (high_order = 1), HRM and NPE (a window
-of high_order recent items)."""
+"""Sequential recommenders on the time-ordered samplers: FPMC and TransRec (high_order = 1), HRM, NPE and FPMCplus (a
+window of high_order recent items)."""

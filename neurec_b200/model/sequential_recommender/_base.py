@@ -37,10 +37,13 @@ class SeqTableRecommender(SeqAbstractRecommender):
         self._data_iter = None
         self._step_loss = None
 
-    def _init_tables(self, shapes):
-        """get_initializer on generator 2017, in the reference's variable order (tf.set_random_seed(2017))."""
-        init = get_initializer(self.init_method, self.stddev, torch.Generator().manual_seed(2017))
-        return [init(s).cuda() for s in shapes]
+    def _init_tables(self, shapes, methods=None):
+        """get_initializer on generator 2017, in the reference's variable order (tf.set_random_seed(2017)).  methods
+        names each shape's initialiser (default: init_method for every shape); all draw from the one generator."""
+        generator = torch.Generator().manual_seed(2017)
+        methods = [self.init_method] * len(shapes) if methods is None else methods
+        inits = {m: get_initializer(m, self.stddev, generator) for m in set(methods)}
+        return [inits[m](s).cuda() for m, s in zip(methods, shapes)]
 
     def _init_training(self, tables):
         self.opt = OptimizerState(self.learner, self.learning_rate)

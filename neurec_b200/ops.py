@@ -1055,6 +1055,73 @@ def npe_train_epoch(UI, IU, IL, users, recent, items, labels, batch_size, loss, 
     return steps
 
 
+# ------------------------------------------------------------------------- FPMCplus: attention over the window
+def fpmcplus_work(dim, weight_size, window, batch_size, device="cuda"):
+    """Zero-filled scratch of the FPMCplus gradient for batches of up to batch_size samples (the dense gradients'
+    per-sample factors, per-chunk partial sums and completion counters)."""
+    n = _lib.load().nrc_fpmcplus_work_floats(int(dim), int(weight_size), int(window), int(batch_size))
+    check(int(n) if n < 0 else 0)
+    return torch.zeros(int(n), dtype=torch.float32, device=device)
+
+
+def fpmcplus_grad(UI, IU, IL, LI, W, b, h, users, recent, items, third, pairwise, loss, reg_mf, reg_w, grads, touched,
+                  stamp, work, loss_out):
+    """Loss + gradients of one FPMCplus batch (FPMCplus.py:53-119); recent i32 [batch, L], grads = (gUI, gIU, gIL, gLI,
+    gW, gb, gh) (the last three dense), touched = (tU, tI, tL)."""
+    check(_lib.load().nrc_fpmcplus_grad(
+        _p(UI), _p(IU), _p(IL), _p(LI), _p(W), _p(b), _p(h), UI.shape[1], W.shape[1], _window(recent), _p(users),
+        _p(recent), _p(items), _p(third), users.numel(), 1 if pairwise else 0, LOSS_IDS[loss], float(reg_mf),
+        float(reg_w), *[_p(g) for g in grads], *[_p(t) for t in touched], int(stamp), _p(work), _p(loss_out),
+        _stream()))
+    _count(2)
+
+
+def fpmcplus_train_epoch(UI, IU, IL, LI, W, b, h, users, recent, items, third, batch_size, pairwise, loss, reg_mf,
+                         reg_w, opt, lr_t, hyper, grads, touched, slots0, slots1, first_stamp, work, step_loss):
+    """One FPMCplus epoch (FPMCplus.py:141-171): grads and slots in the order UI, IU, IL, LI, W, b, h; touched =
+    (tU, tI, tL).  Returns the number of steps."""
+    n, steps, lr_t, hy = _epoch_prologue(users, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_fpmcplus_train_epoch(
+        _p(UI), _p(IU), _p(IL), _p(LI), _p(W), _p(b), _p(h), UI.shape[0], IU.shape[0], UI.shape[1], W.shape[1],
+        _window(recent), _p(users), _p(recent), _p(items), _p(third), n, int(batch_size), 1 if pairwise else 0,
+        LOSS_IDS[loss], float(reg_mf), float(reg_w), OPT_IDS[opt], lr_t.ctypes.data, hy.ctypes.data,
+        *[_p(g) for g in grads], *[_p(t) for t in touched], ctypes.cast(s0, ctypes.c_void_p),
+        ctypes.cast(s1, ctypes.c_void_p), int(first_stamp), _p(work), _p(step_loss), _stream()))
+    _count(3 * steps)
+    return steps
+
+
+def fpmcplus_scores(UI, IU, IL, LI, W, b, h, users, recent, recent_len):
+    """FPMCplus.predict(users, None) on the device: f32 [len(users), num_items].  recent i32 [num_users, L] /
+    recent_len i32 [num_users] hold every user's predict window (see nrc_hrm_query)."""
+    for t, name in ((UI, "UI"), (IU, "IU"), (IL, "IL"), (LI, "LI"), (W, "W"), (b, "b"), (h, "h")):
+        _req(t, torch.float32, name)
+    L, pu, rows, pr, pl = _query_args(users, recent, recent_len)
+    lib = _lib.load()
+    n = lib.nrc_fpmcplus_score_work_floats(IU.shape[0], UI.shape[1], W.shape[1], L, rows)
+    check(int(n) if n < 0 else 0)
+    work = torch.empty(max(int(n), 1), dtype=torch.float32, device=users.device)
+    out = torch.empty((rows, IU.shape[0]), dtype=torch.float32, device=users.device)
+    check(lib.nrc_fpmcplus_scores(_p(UI), _p(IU), _p(IL), _p(LI), _p(W), _p(b), _p(h), IU.shape[0], UI.shape[1],
+                                  W.shape[1], L, pu, rows, pr, pl, _p(work), _p(out), _stream()))
+    _count(2)
+    return out
+
+
+FPMCPLUS_KERNELS = ("grad", "wgrad", "project", "pair")
+FPMCPLUS_ROUTE_FIELDS = ("pairwise", "grid_x", "grid_y", "capped", "window", "rows")
+
+
+def fpmcplus_last_routes():
+    """Routes of the most recent launch of each FPMCplus kernel (nrc_fpmcplus_last_routes) as {kernel: {field:
+    value}}; -1 = no such launch yet or a field the kernel does not decide."""
+    nf = len(FPMCPLUS_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(FPMCPLUS_KERNELS) * nf))()
+    check(_lib.load().nrc_fpmcplus_last_routes(out))
+    return {k: dict(zip(FPMCPLUS_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(FPMCPLUS_KERNELS)}
+
+
 SEQ_KERNELS = ("fpmc_grad", "transrec_grad", "hrm_grad", "npe_grad", "fpmc_scores", "transrec_scores", "hrm_query",
                "npe_query", "npe_relu")
 SEQ_ROUTE_FIELDS = ("pairwise", "session_max", "pre_max", "grid_x", "grid_y", "capped", "window")

@@ -1,4 +1,4 @@
-"""Time of one FPMC, TransRec, HRM and NPE training epoch, and of one full evaluation of each, on the device.
+"""Time of one FPMC, TransRec, HRM, NPE and FPMCplus training epoch, and of one full evaluation of each, on the device.
 
     python profiles/seq_epoch.py OUT_DIR [--repeats 20] [--warmup 3]
 
@@ -9,14 +9,16 @@ high_order = 1, 78 481 at 2 and 77 538 at 3), each model at its conf file's defa
   * TransRec  pairwise bpr (79 424 samples), batch 1024 (78 steps), d 50, adam, reg 0;
   * HRM       high_order 2, max / max pools, cross_entropy, num_neg 4 (392 405 samples), batch 256 (1 533 steps),
               d 16, adam, reg 0;
-  * NPE       high_order 3, cross_entropy, num_neg 4 (387 690 samples), batch 256 (1 515 steps), d 64, adam, reg 0.1.
+  * NPE       high_order 3, cross_entropy, num_neg 4 (387 690 samples), batch 256 (1 515 steps), d 64, adam, reg 0.1;
+  * FPMCplus  high_order 3, pairwise bpr (77 538 samples), batch 128 (606 steps), d 16, weight_size 16, adam,
+              reg_mf 1e-5, reg_w 1e-3.
 Per model, medians over --repeats after --warmup untimed repeats:
   * fused_epoch_ms: CUDA events around the one fused epoch call (nrc_<model>_train_epoch: per batch the gradient
-    kernel and one optimizer launch) on an epoch already on the device;
+    kernel(s) and one optimizer launch) on an epoch already on the device;
   * plug_in_epoch_ms: the plug-in's whole epoch (the sampler's device epoch, Adam's per-step lr_t on the host, the
     fused call, the loss read back), host clock around it;
   * score_kernel_ms: CUDA events around scoring all 943 users x 1 682 items (the score kernel; for HRM and NPE the
-    query kernel and nrc_mf_scores);
+    query kernel and nrc_mf_scores; for FPMCplus the projection pass and the pair kernel);
   * evaluate_ms: the plug-in's evaluation with NeuRec.properties' options (predict in batches of 128 users, train
     items masked, five metrics at top 10 and 20), host clock after a device synchronise.
 The card's name and power limit are read in the same run; the JSON goes to OUT_DIR/seq_epoch.json.
@@ -33,7 +35,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-MODELS = ("FPMC", "TransRec", "HRM", "NPE")
+MODELS = ("FPMC", "TransRec", "HRM", "NPE", "FPMCplus")
 
 
 def card():
@@ -75,10 +77,11 @@ def measure(name, conf, ds, repeats, warmup):
     import torch
     from neurec_b200 import ops
     from neurec_b200.model.sequential_recommender.FPMC import FPMC
+    from neurec_b200.model.sequential_recommender.FPMCplus import FPMCplus
     from neurec_b200.model.sequential_recommender.HRM import HRM
     from neurec_b200.model.sequential_recommender.NPE import NPE
     from neurec_b200.model.sequential_recommender.TransRec import TransRec
-    m = {"FPMC": FPMC, "TransRec": TransRec, "HRM": HRM, "NPE": NPE}[name](None, ds, conf)
+    m = {"FPMC": FPMC, "TransRec": TransRec, "HRM": HRM, "NPE": NPE, "FPMCplus": FPMCplus}[name](None, ds, conf)
     m.build_graph()
     sampler = m.data_iter()
     epoch = sampler.device_epoch()
@@ -96,6 +99,9 @@ def measure(name, conf, ds, repeats, warmup):
         elif name == "TransRec":
             ops.transrec_train_epoch(*m.tables(), *epoch, bs, m.is_pairwise is True, m._loss, reg, *opt, m._work,
                                      step_loss)
+        elif name == "FPMCplus":
+            ops.fpmcplus_train_epoch(*m.tables(), *epoch, bs, m.is_pairwise is True, m._loss, reg, m.reg_w, *opt,
+                                     m._work, step_loss)
         elif name == "HRM":
             ops.hrm_train_epoch(*m.tables(), *epoch, bs, *m._pools(), m._loss, reg, *opt, step_loss)
         else:
