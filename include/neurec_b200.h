@@ -1096,6 +1096,80 @@ int nrc_fpmcplus_scores(const float* ui, const float* iu, const float* il, const
  *   their window rows would not fit in shared memory). */
 int nrc_fpmcplus_last_routes(int32_t* out);
 
+/* ======================================================================================
+ * Caser (model/sequential_recommender/Caser.py): convolutions over the embeddings of the last L items
+ * ==================================================================================== */
+
+/* Caser._create_variable / build_graph, Caser.py:37-122.  Variables P [U, d] (user_embeddings), E [I, d]
+ * (seq_item_embeddings; the pad id I reads a zero row), W2 [I, 2d] (item_embeddings), b2 [I] (item_biases) and the
+ * dense block: every conv and FC weight in one flat f32 buffer, in TF's creation order and layouts,
+ *   Kv [L, 1, 1, nv] (element l nv + f), bv [nv],
+ *   for h = 1..L: Kh_h [h, d, 1, nh] (element (l d + k) nh + f), bh_h [nh],
+ *   W1 [F, d] (element r d + c), b1 [d],           F = nv d + nh L.
+ * One sample is users[b], seqs i32 [batch, L] (the window, oldest first), pos i32 [batch, T] and neg i32 [batch, N]
+ * (N = neg_samples); with X the [L, d] image of the window:
+ *   out_v[k nv + f] = sum_l X[l, k] Kv[l, f] + bv[f],  out_h[(h-1) nh + f] = max_t relu(conv of height h + bh_h[f])
+ *   o = ([out_v, out_h] / keep) * mask (o = [out_v, out_h] when mask is NULL),  z = relu(o W1 + b1)
+ *   x_j = <[z, P_u], W2[j]> + b2[j] over pos ++ neg
+ *   loss = mean(-log(sigmoid(x_pos) + 1e-24)) + mean(-log(1 - sigmoid(x_neg) + 1e-24))   (means over this batch)
+ * A target equal to the pad id I reads a zero row and a zero bias (x = 0): its loss term counts and it gets no
+ * gradient.  Gradients as TF: the max passes grad / n to each of the n tied maxima, relu passes where its output is
+ * > 0.  NRC_E_LIMIT when dim is outside [1, 256], seq_L outside [1, 16], nv or nh outside [1, 64], seq_T +
+ * neg_samples above 64 or batch above 65535 * 32; NRC_E_VALUE when seq_T or neg_samples is below 1, keep is outside
+ * (0, 1] or a table, gradient or work is NULL.  A rejected call writes nothing. */
+
+/* Floats of the dense block (layout above); negative NRC_E_* when a size is out of range. */
+int64_t nrc_caser_dense_floats(int32_t dim, int32_t seq_L, int32_t nv, int32_t nh);
+
+/* Scratch of nrc_caser_grad / nrc_caser_train_epoch in floats, for batches of up to batch_size samples: completion
+ * counters, each sample's layer inputs and output gradients, per-chunk partial sums of the dense gradient and the
+ * step's dropout mask.  Zero-fill it once before its first use; every call leaves the counters ready for the next
+ * (calls that share one work buffer must not run concurrently). */
+int64_t nrc_caser_work_floats(int32_t dim, int32_t seq_L, int32_t nv, int32_t nh, int32_t batch_size);
+
+/* Loss and gradients of one batch.  mask f32 [batch, F] (0 / 1) applies dropout with keep probability keep; NULL
+ * means no dropout.  Row gradients are ADDED into grad_user [U, d], grad_seq [I, d] (window rows; pad ids get none),
+ * grad_item [I, 2d] and grad_bias [I] (targets) with atomics; grad_dense [dense floats] is OVERWRITTEN with the
+ * dense block's gradient, summed over the batch in one fixed order (the same bits on every call).  The batch's data
+ * loss (without the l2 term) is ADDED into *loss when loss is not NULL. */
+int nrc_caser_grad(const float* user_table, const float* seq_table, const float* item_table, const float* item_bias,
+                   const float* dense, int32_t num_items, int32_t dim, int32_t seq_L, int32_t seq_T, int32_t nv,
+                   int32_t nh, int32_t neg_samples, const int32_t* users, const int32_t* seqs, const int32_t* pos,
+                   const int32_t* neg, int64_t batch, const float* mask, float keep, float* grad_user,
+                   float* grad_seq, float* grad_item, float* grad_bias, float* grad_dense, float* work, float* loss,
+                   void* stream);
+
+/* Caser.train_model's batch loop, Caser.py:128-139, over an epoch already shuffled and sampled (users, seqs, pos,
+ * neg as above, n samples).  Per batch s: the dropout mask nrc_dropout_mask(rows * F, keep, seed, epoch << 32 | s);
+ * every table's gradient set to l2_reg * var (0 when l2_reg = 0); nrc_caser_grad; one Adam launch (hyper_host =
+ * {lr, beta1, beta2, eps}, lr_t_host [steps]) over P, E, W2, b2 in the IndexedSlices form on every row and the
+ * dense block in the dense form.  slot0 / slot1: HOST arrays of the five variables' m and v slots in that order.
+ * step_loss f32 [steps] gets each batch's data loss. */
+int nrc_caser_train_epoch(float* user_table, float* seq_table, float* item_table, float* item_bias, float* dense,
+                          int32_t num_users, int32_t num_items, int32_t dim, int32_t seq_L, int32_t seq_T, int32_t nv,
+                          int32_t nh, int32_t neg_samples, const int32_t* users, const int32_t* seqs,
+                          const int32_t* pos, const int32_t* neg, int64_t n, int32_t batch_size, float keep,
+                          float l2_reg, uint64_t seed, uint64_t epoch, const float* lr_t_host,
+                          const float* hyper_host, float* grad_user, float* grad_seq, float* grad_item,
+                          float* grad_bias, float* grad_dense, float* const* slot0, float* const* slot1, float* work,
+                          float* step_loss, void* stream);
+
+/* Caser.predict's user vectors, Caser.py:194-209: out f32 [rows, 2d] = [z, P_u] of user users[r] without dropout,
+ * over its window windows[users[r]] (windows i32 [num_users, L]).  The scores of every item are
+ * nrc_mf_scores(out, W2) -- the reference's all_logits, without b2. */
+int nrc_caser_query(const float* user_table, const float* seq_table, const float* dense, int32_t num_items,
+                    int32_t dim, int32_t seq_L, int32_t nv, int32_t nh, const int32_t* users, int64_t rows,
+                    const int32_t* windows, float* out, void* stream);
+
+/* Test hook of the Caser kernels, as nrc_seq_last_routes: out i32[4 * 6], group k at out[6 * k].
+ *   groups: [0] the per-sample gradient kernel, [1] the dense-gradient reduction (both also inside
+ *   nrc_caser_train_epoch), [2] the query kernel, [3] the per-step reg pass of nrc_caser_train_epoch.
+ *   fields: +0 1 when the dense block was staged in shared memory (it fits with the kernel's buffers), 0 when it was
+ *   read from global memory; +1 gridDim.x (CTAs; the reduction: element tiles of 256); +2 gridDim.y (the reduction:
+ *   chunks of 32 samples); +3 1 when the grid was capped (the gradient and query kernels above 2 * SMs samples or
+ *   rows, the reg pass above 4096 * SMs elements), else 0; +4 the window L; +5 1 when a dropout mask was applied. */
+int nrc_caser_last_routes(int32_t* out);
+
 /* Test hook of the sequential kernels (it reports and changes nothing; every route is chosen by the shape).
  * nrc_seq_last_routes: HOST bookkeeping of the most recent launch of each kernel group, written when a call launches
  * (a call that returns before launching, for a failed check, an empty batch or no rows, leaves it as it was); one

@@ -1122,6 +1122,84 @@ def fpmcplus_last_routes():
     return {k: dict(zip(FPMCPLUS_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(FPMCPLUS_KERNELS)}
 
 
+# ------------------------------------------------------------------------- Caser: convolutions over the window
+def caser_dense_floats(dim, seq_L, nv, nh):
+    """Floats of Caser's dense block (every conv and FC weight and bias, layout in nrc_caser_dense_floats)."""
+    n = _lib.load().nrc_caser_dense_floats(int(dim), int(seq_L), int(nv), int(nh))
+    check(int(n) if n < 0 else 0)
+    return int(n)
+
+
+def caser_work(dim, seq_L, nv, nh, batch_size, device="cuda"):
+    """Zero-filled scratch of the Caser gradient and epoch for batches of up to batch_size samples."""
+    n = _lib.load().nrc_caser_work_floats(int(dim), int(seq_L), int(nv), int(nh), int(batch_size))
+    check(int(n) if n < 0 else 0)
+    return torch.zeros(int(n), dtype=torch.float32, device=device)
+
+
+def _caser_sizes(P, W2, seqs, nv, nh):
+    return P.shape[1], _window(seqs), int(nv), int(nh), W2.shape[0]
+
+
+def caser_grad(P, E, W2, b2, dense, users, seqs, pos, neg, nv, nh, mask, keep, grads, work, loss_out=None):
+    """Loss and gradients of one Caser batch (Caser.py:70-118): seqs i32 [batch, L], pos i32 [batch, T], neg i32
+    [batch, N], mask f32 [batch, F] or None; grads = (gP, gE, gW2, gb2) accumulated, gDense overwritten."""
+    d, L, nv, nh, ni = _caser_sizes(P, W2, seqs, nv, nh)
+    check(_lib.load().nrc_caser_grad(
+        _p(P), _p(E), _p(W2), _p(b2), _p(dense), ni, d, L, pos.shape[1], nv, nh, neg.shape[1], _p(users), _p(seqs),
+        _p(pos), _p(neg), users.numel(), _p(mask), float(keep), *[_p(g) for g in grads], _p(work), _p(loss_out),
+        _stream()))
+    _count(2)
+
+
+def caser_train_epoch(P, E, W2, b2, dense, users, seqs, pos, neg, nv, nh, batch_size, keep, l2_reg, seed, epoch, lr_t,
+                      hyper, grads, slots0, slots1, work, step_loss):
+    """One Caser epoch (Caser.py:128-139) over an already shuffled and sampled epoch: grads and slots in the order
+    P, E, W2, b2, dense.  Returns the number of steps."""
+    d, L, nv, nh, ni = _caser_sizes(P, W2, seqs, nv, nh)
+    n, steps, lr_t, hy = _epoch_prologue(users, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_caser_train_epoch(
+        _p(P), _p(E), _p(W2), _p(b2), _p(dense), P.shape[0], ni, d, L, pos.shape[1], nv, nh, neg.shape[1], _p(users),
+        _p(seqs), _p(pos), _p(neg), n, int(batch_size), float(keep), float(l2_reg), int(seed), int(epoch),
+        lr_t.ctypes.data, hy.ctypes.data, *[_p(g) for g in grads], ctypes.cast(s0, ctypes.c_void_p),
+        ctypes.cast(s1, ctypes.c_void_p), _p(work), _p(step_loss), _stream()))
+    _count(5 * steps)
+    return steps
+
+
+def caser_query(P, E, W2, dense, users, windows, nv, nh):
+    """Caser.predict's user vectors [z, P_u] (Caser.py:194-209): f32 [len(users), 2d] over windows i32 [num_users, L]."""
+    for t, name in ((P, "P"), (E, "E"), (W2, "W2"), (dense, "dense")):
+        _req(t, torch.float32, name)
+    _req(users, torch.int32, "users"); _req(windows, torch.int32, "windows")
+    d, L, nv, nh, ni = _caser_sizes(P, W2, windows, nv, nh)
+    out = torch.empty((users.numel(), 2 * d), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_caser_query(_p(P), _p(E), _p(dense), ni, d, L, nv, nh, _p(users), users.numel(),
+                                      _p(windows), _p(out), _stream()))
+    _count()
+    return out
+
+
+def caser_scores(P, E, W2, dense, users, windows, nv, nh):
+    """Caser.predict(users, None) on the device: f32 [len(users), num_items], [z, P_u] W2^T without the biases."""
+    q = caser_query(P, E, W2, dense, users, windows, nv, nh)
+    return mf_scores(q, W2, torch.arange(users.numel(), dtype=torch.int32, device=users.device))
+
+
+CASER_KERNELS = ("grad", "wgrad", "query", "reg")
+CASER_ROUTE_FIELDS = ("staged", "grid_x", "grid_y", "capped", "window", "masked")
+
+
+def caser_last_routes():
+    """Routes of the most recent launch of each Caser kernel (nrc_caser_last_routes) as {kernel: {field: value}};
+    -1 = no such launch yet or a field the kernel does not decide."""
+    nf = len(CASER_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(CASER_KERNELS) * nf))()
+    check(_lib.load().nrc_caser_last_routes(out))
+    return {k: dict(zip(CASER_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(CASER_KERNELS)}
+
+
 SEQ_KERNELS = ("fpmc_grad", "transrec_grad", "hrm_grad", "npe_grad", "fpmc_scores", "transrec_scores", "hrm_query",
                "npe_query", "npe_relu")
 SEQ_ROUTE_FIELDS = ("pairwise", "session_max", "pre_max", "grid_x", "grid_y", "capped", "window")
