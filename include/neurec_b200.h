@@ -1190,6 +1190,27 @@ int nrc_caser_last_routes(int32_t* out);
  *   +6 the window L (HRM and NPE). */
 int nrc_seq_last_routes(int32_t* out);
 
+/* Test hook of the data-side kernels (APR's normaliser, the row gather, SBPR, the CSR / split / row-id builders), the
+ * negative samplers and LightGCN's BPR gradient (it reports and changes nothing; every route is chosen by the shape).
+ * nrc_extras_last_routes: HOST bookkeeping of the most recent launch of each group, written just before the launch (a
+ * call that returns before launching, for a failed check or an empty input, leaves it as it was); one record per
+ * process.  out i32[10 * 6], group k at out[6 * k]; -1 = no such launch yet, or a field the group does not decide.
+ *   groups: [0] nrc_l2_normalize_rows, [1] nrc_gather_rows_i32, [2] nrc_sbpr_epoch_build, [3] nrc_sbpr_grad (also
+ *   inside nrc_sbpr_train_epoch), [4] nrc_csr_from_coo, [5] nrc_split_interactions, [6] nrc_csr_row_ids,
+ *   [7] nrc_sample_negatives, [8] nrc_batch_randint_choice, [9] nrc_lightgcn_bpr_grad (also inside
+ *   nrc_lightgcn_train_epoch).
+ *   fields of a group:
+ *   +0 CTAs launched (gridDim.x); [4] and [5]: of the per-entry passes (count, scatter), 0 when there are no entries;
+ *   +1 1 when that grid was capped, so a thread or warp takes more than one item, else 0: the per-row kernels ([0],
+ *      [3], [6], [9]) above 64 * SMs rows or samples, the per-element kernels ([1], [2], the entry passes of [4] and
+ *      [5]) above 2048 * SMs elements, the samplers' per-element kernels above 4096 * SMs; the no-replace form of [8]
+ *      (one thread per row) is never capped;
+ *   +2 [4], [5]: CTAs of the per-row passes (sort and compaction, split ranks), a warp per row;
+ *   +3 [4], [5]: 1 when the per-row grid was capped (above 64 * SMs rows), else 0;
+ *   +4 [4], [5]: 1024-row chunks of the single-CTA row-pointer scan, ceil(rows / 1024);
+ *   +5 [8]: 1 the replace form, 0 the no-replace form. */
+int nrc_extras_last_routes(int32_t* out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,6 +15,7 @@
 // s_uk = 1 + #{trusted f : social item in train(f)} (SBPR.py:141-145).
 #include "common.cuh"
 #include "epoch.cuh"
+#include "extras.cuh"
 #include "learner.cuh"
 #include "optim.cuh"
 #include "philox.cuh"
@@ -336,6 +337,24 @@ static unsigned grid_for(int64_t work_items, int per_block) {
     return (unsigned)blocks;
 }
 
+// 1 when grid_for capped the grid, so a thread (per_block 256) or warp (per_block 8) takes more than one item
+static int grid_capped(int64_t work_items, int per_block) {
+    return (work_items + per_block - 1) / per_block > (int64_t)sm_count() * 8 ? 1 : 0;
+}
+
+// Host record of the most recent launch of each kernel group, for nrc_extras_last_routes (see the header).
+static struct ExtrasRoutes {
+    int32_t r[kExKernels][kExFields];
+    ExtrasRoutes() { for (auto& k : r) for (auto& f : k) f = -1; }
+} g_extras_routes;
+
+void extras_route(int kernel, int64_t grid, int capped, int64_t row_grid, int row_capped, int64_t scan_chunks,
+                  int replace) {
+    int32_t* r = g_extras_routes.r[kernel];
+    r[kExGrid] = (int32_t)grid; r[kExCapped] = capped; r[kExRowGrid] = (int32_t)row_grid; r[kExRowCapped] = row_capped;
+    r[kExScanChunks] = (int32_t)scan_chunks; r[kExReplace] = replace;
+}
+
 static int sbpr_spec_init(SbprSpec& S, const int64_t* tptr, const int32_t* tidx, const int64_t* sptr, const int32_t* sidx,
                           const int64_t* fptr, const int32_t* fidx, const int32_t* users, const int32_t* pos, int64_t n,
                           int32_t num_items, int32_t max_excluded, int32_t shuffle, uint64_t seed, uint64_t epoch) {
@@ -355,6 +374,7 @@ extern "C" int nrc_l2_normalize_rows(const float* x, int64_t rows, int32_t dim, 
     NRC_REQUIRE(rows >= 0 && dim > 0, NRC_E_VALUE, "bad table shape");
     if (rows == 0) return NRC_OK;
     NRC_REQUIRE(x && out, NRC_E_VALUE, "NULL table");
+    extras_route(kExL2Normalize, grid_for(rows, 8), grid_capped(rows, 8));
     l2_normalize_rows_kernel<<<grid_for(rows, 8), 256, 0, as_stream(stream)>>>(x, out, rows, dim, scale);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
@@ -364,6 +384,7 @@ extern "C" int nrc_gather_rows_i32(const int32_t* src, int64_t src_rows, int32_t
                                    int32_t* out, void* stream) {
     NRC_REQUIRE(src_rows > 0 && width > 0 && n >= 0, NRC_E_VALUE, "bad gather shape");
     if (n == 0) return NRC_OK;
+    extras_route(kExGatherRows, grid_for(n * width, 256), grid_capped(n * width, 256));
     gather_rows_i32_kernel<<<grid_for(n * width, 256), 256, 0, as_stream(stream)>>>(src, src_rows, width, index, n, out);
     NRC_CUDA_CHECK(cudaGetLastError());
     return NRC_OK;
@@ -382,6 +403,7 @@ extern "C" int nrc_sbpr_epoch_build(const int64_t* train_indptr, const int32_t* 
     NRC_REQUIRE(first >= 0 && count >= 0 && first + count <= n_pos, NRC_E_VALUE, "window [%lld, %lld) outside the epoch of %lld samples",
                 (long long)first, (long long)(first + count), (long long)n_pos);
     if (count == 0) return NRC_OK;
+    extras_route(kExSbprEpochBuild, grid_for(count, 256), grid_capped(count, 256));
     sbpr_epoch_build_kernel<<<grid_for(count, 256), 256, 0, as_stream(stream)>>>(S, first, count, out_users, out_pos, out_social,
                                                                                   out_neg, out_suk);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -397,6 +419,7 @@ extern "C" int nrc_sbpr_grad(const float* user_table, const float* item_table, c
     // learner.py:27-28
     NRC_REQUIRE(loss_kind >= NRC_LOSS_BPR && loss_kind <= NRC_LOSS_SQUARE, NRC_E_VALUE, "please choose a suitable loss function");
     if (batch == 0) return NRC_OK;
+    extras_route(kExSbprGrad, grid_for(batch, 8), grid_capped(batch, 8));
     sbpr_grad_kernel<<<grid_for(batch, 8), 256, 0, as_stream(stream)>>>(user_table, item_table, item_bias, dim, users, pos_items,
                                                                          social_items, neg_items, suk, batch, loss_kind, reg,
                                                                          grad_user, grad_item, grad_bias, touched_user,
@@ -459,6 +482,8 @@ extern "C" int nrc_csr_from_coo(const int32_t* rows, const int32_t* cols, int64_
     NRC_CUDA_CHECK(cudaMemsetAsync(cursor, 0, (size_t)(num_rows + 1) * 8, st));
     NRC_CUDA_CHECK(cudaMemsetAsync(out_indptr, 0, (size_t)(num_rows + 1) * 8, st));
     NRC_CUDA_CHECK(cudaMemsetAsync(bad_flag, 0, 4, st));
+    extras_route(kExCsrFromCoo, nnz ? grid_for(nnz, 256) : 0, nnz ? grid_capped(nnz, 256) : 0, grid_for(num_rows, 8),
+                 grid_capped(num_rows, 8), ((int64_t)num_rows + 1023) / 1024);
     if (nnz) coo_count_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(rows, cols, nnz, num_rows, num_cols, raw_ptr, bad_flag);
     scan_i64_kernel<<<1, 1024, 0, st>>>(raw_ptr, num_rows);
     if (nnz) coo_scatter_kernel<<<grid_for(nnz, 256), 256, 0, st>>>(rows, cols, nnz, num_rows, num_cols, raw_ptr, cursor, scattered);
@@ -486,6 +511,8 @@ extern "C" int nrc_split_interactions(const int32_t* users, const int64_t* keys,
     NRC_CUDA_CHECK(cudaMemsetAsync(cursor, 0, (size_t)(num_users + 1) * 8, st));
     NRC_CUDA_CHECK(cudaMemsetAsync(bad_flag, 0, 4, st));
     if (n == 0) return NRC_OK;
+    extras_route(kExSplit, grid_for(n, 256), grid_capped(n, 256), grid_for(num_users, 8), grid_capped(num_users, 8),
+                 ((int64_t)num_users + 1023) / 1024);
     coo_count_rows_kernel<<<grid_for(n, 256), 256, 0, st>>>(users, n, num_users, ptr, bad_flag);
     scan_i64_kernel<<<1, 1024, 0, st>>>(ptr, num_users);
     index_scatter_kernel<<<grid_for(n, 256), 256, 0, st>>>(users, n, num_users, ptr, cursor, work_i32);
@@ -499,7 +526,17 @@ extern "C" int nrc_split_interactions(const int32_t* users, const int64_t* keys,
 extern "C" int nrc_csr_row_ids(const int64_t* indptr, int64_t num_rows, int32_t* out, void* stream) {
     NRC_REQUIRE(num_rows >= 0, NRC_E_VALUE, "num_rows >= 0 required");
     if (num_rows == 0) return NRC_OK;
+    extras_route(kExCsrRowIds, grid_for(num_rows, 8), grid_capped(num_rows, 8));
     csr_row_ids_kernel<<<grid_for(num_rows, 8), 256, 0, as_stream(stream)>>>(indptr, num_rows, out);
     NRC_CUDA_CHECK(cudaGetLastError());
+    return NRC_OK;
+}
+
+// Host bookkeeping of the routes the most recent data-side, sampler and LightGCN-gradient launches took (see the
+// header); no device work.
+extern "C" int nrc_extras_last_routes(int32_t* out) {
+    NRC_REQUIRE(out != nullptr, NRC_E_VALUE, "out is NULL");
+    for (int k = 0; k < kExKernels; ++k)
+        for (int f = 0; f < kExFields; ++f) out[k * kExFields + f] = g_extras_routes.r[k][f];
     return NRC_OK;
 }

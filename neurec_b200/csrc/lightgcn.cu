@@ -22,6 +22,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "extras.cuh"
 #include "graph.cuh"
 #include "learner.cuh"
 #include "optim.cuh"
@@ -439,7 +440,9 @@ extern "C" int nrc_lightgcn_bpr_grad(const float* e_final, const float* e0, int3
     if (batch == 0) return NRC_OK;
     int64_t blocks = (batch + 7) / 8;
     const int64_t cap = (int64_t)sm_count() * 8;
+    const int capped = blocks > cap ? 1 : 0;
     if (blocks > cap) blocks = cap;
+    extras_route(kExLightgcnGrad, blocks, capped);
     lightgcn_grad_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(
         e_final, e0, num_users, dim, users, pos_items, neg_items, batch, reg, scale, grad_final,
         grad_reg, loss2);

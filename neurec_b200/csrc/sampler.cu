@@ -14,6 +14,7 @@
 // exactly like `llrand() % high` (random_choice.pyx:53).  oracle/neurec_oracle.c restates this
 // generator on the CPU; tests require bit-equality.
 #include "common.cuh"
+#include "extras.cuh"
 #include "philox.cuh"
 
 namespace nrc {
@@ -98,7 +99,9 @@ extern "C" int nrc_sample_negatives(const int64_t* train_indptr, const int32_t* 
     const int threads = 256;
     int64_t blocks = (total + threads - 1) / threads;
     const int64_t cap = (int64_t)sm_count() * 16;
+    const int capped = blocks > cap ? 1 : 0;
     if (blocks > cap) blocks = cap;
+    extras_route(kExSampleNegatives, blocks, capped);
     sample_negatives_kernel<<<(unsigned)blocks, threads, 0, as_stream(stream)>>>(
         train_indptr, train_indices, users, n, neg_num, num_items, seed, stream_id, first_index, out);
     NRC_CUDA_CHECK(cudaGetLastError());
@@ -117,10 +120,13 @@ extern "C" int nrc_batch_randint_choice(int32_t high, const int64_t* out_indptr,
     if (replace) {
         int64_t blocks = (total_out + threads - 1) / threads;
         const int64_t cap = (int64_t)sm_count() * 16;
+        const int capped = blocks > cap ? 1 : 0;
         if (blocks > cap) blocks = cap;
+        extras_route(kExBatchChoice, blocks, capped, -1, -1, -1, 1);
         batch_choice_replace_kernel<<<(unsigned)blocks, threads, 0, as_stream(stream)>>>(
             high, out_indptr, n_rows, total_out, excl_indptr, excl_indices, seed, stream_id, out);
     } else {
+        extras_route(kExBatchChoice, (n_rows + threads - 1) / threads, 0, -1, -1, -1, 0);
         batch_choice_noreplace_kernel<<<(n_rows + threads - 1) / threads, threads, 0,
                                         as_stream(stream)>>>(high, out_indptr, n_rows, excl_indptr,
                                                              excl_indices, seed, stream_id, out);

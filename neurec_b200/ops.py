@@ -1214,6 +1214,20 @@ def seq_last_routes():
     return {k: dict(zip(SEQ_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(SEQ_KERNELS)}
 
 
+EXTRAS_KERNELS = ("l2_normalize_rows", "gather_rows_i32", "sbpr_epoch_build", "sbpr_grad", "csr_from_coo",
+                  "split_interactions", "csr_row_ids", "sample_negatives", "batch_randint_choice", "lightgcn_bpr_grad")
+EXTRAS_ROUTE_FIELDS = ("grid", "capped", "row_grid", "row_capped", "scan_chunks", "replace")
+
+
+def extras_last_routes():
+    """Routes of the most recent launch of each data-side, sampler and LightGCN-gradient kernel group
+    (nrc_extras_last_routes) as {kernel: {field: value}}; -1 = no such launch yet or a field the group does not decide."""
+    nf = len(EXTRAS_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(EXTRAS_KERNELS) * nf))()
+    check(_lib.load().nrc_extras_last_routes(out))
+    return {k: dict(zip(EXTRAS_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(EXTRAS_KERNELS)}
+
+
 def csr_from_coo(rows, cols, num_rows, num_cols):
     """Interactions -> (indptr i64 [num_rows + 1], indices i32 [distinct]) with ascending duplicate-free rows
     (Dataset.to_csr_matrix + csr_to_user_dict, dataset.py:288-296, tool.py:56-65).  ValueError on ids out of range."""
