@@ -1170,6 +1170,67 @@ int nrc_caser_query(const float* user_table, const float* seq_table, const float
  *   rows, the reg pass above 4096 * SMs elements), else 0; +4 the window L; +5 1 when a dropout mask was applied. */
 int nrc_caser_last_routes(int32_t* out);
 
+/* ======================================================================================
+ * FISM (model/general_recommender/FISM.py): a user is the sum of the item rows of its train history
+ * ==================================================================================== */
+
+/* FISM._create_variables / _create_inference / _create_loss, FISM.py:55-88.  Variables c1 [I, d], Q [I, d]
+ * (embedding_Q) and b [I] (bias).  Histories are rows of a CSR (hist_ptr i64 [rows + 1], hist_idx i32); the
+ * reference's pad id (a zero row) is not materialised.  Sample s is (rows[s], excl[s], num[s], items[s], third[s]):
+ *   p = sum of c1[h] over h in hist_idx[hist_ptr[r] .. hist_ptr[r + 1]) with h != excl[s] (excl NULL or -1: none)
+ *   x = powf(num[s], -alpha) * <p, Q[i]> + b[i]
+ *   pointwise (third = labels f32):    l(z, x) + lambda * l2_loss(p) + gamma * l2_loss(Q[i])
+ *   pairwise  (third = negatives i32): l(x - x_j) + lambda * l2_loss(p) + gamma * (l2_loss(Q[j]) + l2_loss(Q[i])),
+ *     x_j = powf(num_neg[s], -alpha) * <p, Q[j]> + b[j] over the same history p.
+ * l2_loss(t) = sum t^2 / 2.  Cross entropy is a batch mean, the other losses are sums.  Every history row h (once per
+ * occurrence; once for both sides of a pair) takes dl/dp = g c Q[i] [- g c_j Q[j]] + lambda p.  NRC_E_LIMIT when dim
+ * is outside [1, 256]; NRC_E_VALUE when num_items < 1, the loss does not suit the mode, batch < 0, alpha is not
+ * finite, or a table, the CSR, the batch, num_neg (pairwise), a gradient or a stamp array is NULL.  A rejected call
+ * writes nothing. */
+
+/* Loss and row gradients of one batch.  Gradients are ADDED into grad_c1 [I, d], grad_q [I, d] and grad_bias [I] with
+ * atomics; touched_c1[h] = stamp for every history row read, touched_item[i] (and [j]) = stamp for the targets (Q and
+ * b share it).  The batch's loss, regularisers included, is ADDED into *loss when loss is not NULL. */
+int nrc_fism_grad(const float* c1, const float* q, const float* bias, int32_t num_items, int32_t dim,
+                  const int64_t* hist_ptr, const int32_t* hist_idx, const int32_t* rows, const int32_t* excl,
+                  const int32_t* num, const int32_t* items, const void* third, const int32_t* num_neg, int64_t batch,
+                  int32_t pairwise, int32_t loss_kind, float alpha, float lambda, float gamma, float* grad_c1,
+                  float* grad_q, float* grad_bias, int32_t* touched_c1, int32_t* touched_item, int32_t stamp,
+                  float* loss, void* stream);
+
+/* FISM.train_model's batch loop, FISM.py:100-144, over an epoch already built and shuffled (n samples as above).  Per
+ * batch s (stamp first_stamp + s): nrc_fism_grad, then one optimizer launch over c1, Q and b, all three in the
+ * IndexedSlices form (touched rows for adagrad / rmsprop / momentum, Adam's sparse form on every row).  lr_t_host
+ * [steps] is Adam's lr_t per step (ignored otherwise); hyper_host = {lr, beta1 | rho | momentum, beta2 | momentum,
+ * eps}; slot0 / slot1: HOST arrays of the three variables' slots (NULL entries where the optimizer keeps none).
+ * step_loss f32 [steps] gets each batch's loss. */
+int nrc_fism_train_epoch(float* c1, float* q, float* bias, int32_t num_items, int32_t dim, const int64_t* hist_ptr,
+                         const int32_t* hist_idx, const int32_t* rows, const int32_t* excl, const int32_t* num,
+                         const int32_t* items, const void* third, const int32_t* num_neg, int64_t n,
+                         int32_t batch_size, int32_t pairwise, int32_t loss_kind, float alpha, float lambda,
+                         float gamma, int32_t opt_kind, const float* lr_t_host, const float* hyper_host,
+                         float* grad_c1, float* grad_q, float* grad_bias, int32_t* touched_c1, int32_t* touched_item,
+                         float* const* slot0, float* const* slot1, int32_t first_stamp, float* step_loss,
+                         void* stream);
+
+/* FISM.predict's user rows, FISM.py:154-180: out f32 [rows, d] = the sum of c1 over user users[r]'s whole history
+ * row. */
+int nrc_fism_query(const float* c1, int32_t num_items, int32_t dim, const int64_t* hist_ptr, const int32_t* hist_idx,
+                   const int32_t* users, int64_t rows, float* out, void* stream);
+
+/* Scores of every item: out f32 [rows, I], out[r, j] = powf(n, -alpha) * <query[r], Q[j]> + b[j] with n the length
+ * of user users[r]'s history row (query from nrc_fism_query).  NRC_E_LIMIT also when I is above 65535 * 256. */
+int nrc_fism_scores(const float* query, const float* q, const float* bias, int32_t num_items, int32_t dim, float alpha,
+                    const int64_t* hist_ptr, const int32_t* users, int64_t rows, float* out, void* stream);
+
+/* Test hook of the FISM kernels, as nrc_seq_last_routes: out i32[3 * 6], group k at out[6 * k].
+ *   groups: [0] the gradient kernel (also inside nrc_fism_train_epoch), [1] the query kernel, [2] the score kernel.
+ *   fields: +0 1 the pairwise form, 0 the pointwise one (gradient); +1 floats per lane load (4 when dim % 4 == 0,
+ *   else 1); +2 lanes per history row (gradient and query: a power of two, 32 / lanes rows per warp load); +3
+ *   gridDim.x (CTAs of 64 threads, a warp per sample or row; the score kernel: groups of 8 rows); +4 gridDim.y (the
+ *   score kernel: item tiles of 256); +5 1 when the grid was capped above 64 * SMs samples or rows, else 0. */
+int nrc_fism_last_routes(int32_t* out);
+
 /* Test hook of the sequential kernels (it reports and changes nothing; every route is chosen by the shape).
  * nrc_seq_last_routes: HOST bookkeeping of the most recent launch of each kernel group, written when a call launches
  * (a call that returns before launching, for a failed check, an empty batch or no rows, leaves it as it was); one

@@ -1200,6 +1200,87 @@ def caser_last_routes():
     return {k: dict(zip(CASER_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(CASER_KERNELS)}
 
 
+# ------------------------------------------------------------------------- FISM: item similarity over the history
+def _fism_samples(hist_ptr, hist_idx, rows, excl, num, items, third, num_neg, pairwise):
+    _req(hist_ptr, torch.int64, "hist_ptr"); _req(hist_idx, torch.int32, "hist_idx")
+    for t, name in ((rows, "rows"), (num, "num"), (items, "items")):
+        _req(t, torch.int32, name)
+    if excl is not None:
+        _req(excl, torch.int32, "excl")
+    _req(third, torch.int32 if pairwise else torch.float32, "third")
+    if pairwise:
+        _req(num_neg, torch.int32, "num_neg")
+    return rows.numel()
+
+
+def fism_grad(c1, Q, b, hist_ptr, hist_idx, rows, excl, num, items, third, num_neg, pairwise, loss, alpha, lam, gamma,
+              grads, touched, stamp, loss_out=None):
+    """Loss and row gradients of one FISM batch (FISM.py:69-94): sample s sums c1 over history row rows[s] of the CSR
+    (hist_ptr, hist_idx) without item excl[s] (excl None or -1: none); `third` = negatives (i32, pairwise, with
+    num_neg their counts) or labels (f32).  grads = (gC1, gQ, gb) and touched = (tC1, tItem) are accumulated."""
+    n = _fism_samples(hist_ptr, hist_idx, rows, excl, num, items, third, num_neg, pairwise)
+    check(_lib.load().nrc_fism_grad(
+        _p(c1), _p(Q), _p(b), Q.shape[0], Q.shape[1], _p(hist_ptr), _p(hist_idx), _p(rows), _p(excl), _p(num),
+        _p(items), _p(third), _p(num_neg) if pairwise else None, n, 1 if pairwise else 0, LOSS_IDS[loss],
+        float(alpha), float(lam), float(gamma), *[_p(g) for g in grads], *[_p(t) for t in touched], int(stamp),
+        _p(loss_out), _stream()))
+    _count()
+
+
+def fism_train_epoch(c1, Q, b, hist_ptr, hist_idx, rows, excl, num, items, third, num_neg, batch_size, pairwise, loss,
+                     alpha, lam, gamma, opt, lr_t, hyper, grads, touched, slots0, slots1, first_stamp, step_loss):
+    """One FISM epoch (FISM.py:112-138) over an already built and shuffled epoch: grads, slots in the order c1, Q, b;
+    touched = (tC1, tItem).  Returns the number of steps."""
+    _fism_samples(hist_ptr, hist_idx, rows, excl, num, items, third, num_neg, pairwise)
+    n, steps, lr_t, h = _epoch_prologue(rows, batch_size, lr_t, hyper)
+    s0, s1 = _slot_array(slots0), _slot_array(slots1)
+    check(_lib.load().nrc_fism_train_epoch(
+        _p(c1), _p(Q), _p(b), Q.shape[0], Q.shape[1], _p(hist_ptr), _p(hist_idx), _p(rows), _p(excl), _p(num),
+        _p(items), _p(third), _p(num_neg) if pairwise else None, n, int(batch_size), 1 if pairwise else 0,
+        LOSS_IDS[loss], float(alpha), float(lam), float(gamma), OPT_IDS[opt], lr_t.ctypes.data, h.ctypes.data,
+        *[_p(g) for g in grads], *[_p(t) for t in touched], ctypes.cast(s0, ctypes.c_void_p),
+        ctypes.cast(s1, ctypes.c_void_p), int(first_stamp), _p(step_loss), _stream()))
+    _count(2 * steps)
+    return steps
+
+
+def fism_query(c1, hist_ptr, hist_idx, users):
+    """FISM.predict's user rows (FISM.py:154-180): f32 [len(users), d], the sum of c1 over each user's history row."""
+    _req(c1, torch.float32, "c1"); _req(hist_ptr, torch.int64, "hist_ptr"); _req(hist_idx, torch.int32, "hist_idx")
+    _req(users, torch.int32, "users")
+    out = torch.empty((users.numel(), c1.shape[1]), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_fism_query(_p(c1), c1.shape[0], c1.shape[1], _p(hist_ptr), _p(hist_idx), _p(users),
+                                     users.numel(), _p(out), _stream()))
+    _count()
+    return out
+
+
+def fism_scores(c1, Q, b, hist_ptr, hist_idx, users, alpha):
+    """FISM.predict(users, None) on the device: f32 [len(users), num_items], n^(-alpha) <p_u, Q_j> + b_j with n the
+    length of the user's history row."""
+    for t, name in ((Q, "Q"), (b, "b")):
+        _req(t, torch.float32, name)
+    p = fism_query(c1, hist_ptr, hist_idx, users)
+    out = torch.empty((users.numel(), Q.shape[0]), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_fism_scores(_p(p), _p(Q), _p(b), Q.shape[0], Q.shape[1], float(alpha), _p(hist_ptr),
+                                      _p(users), users.numel(), _p(out), _stream()))
+    _count()
+    return out
+
+
+FISM_KERNELS = ("grad", "query", "scores")
+FISM_ROUTE_FIELDS = ("pairwise", "vec", "lanes", "grid_x", "grid_y", "capped")
+
+
+def fism_last_routes():
+    """Routes of the most recent launch of each FISM kernel (nrc_fism_last_routes) as {kernel: {field: value}};
+    -1 = no such launch yet or a field the kernel does not decide."""
+    nf = len(FISM_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(FISM_KERNELS) * nf))()
+    check(_lib.load().nrc_fism_last_routes(out))
+    return {k: dict(zip(FISM_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(FISM_KERNELS)}
+
+
 SEQ_KERNELS = ("fpmc_grad", "transrec_grad", "hrm_grad", "npe_grad", "fpmc_scores", "transrec_scores", "hrm_query",
                "npe_query", "npe_relu")
 SEQ_ROUTE_FIELDS = ("pairwise", "session_max", "pre_max", "grid_x", "grid_y", "capped", "window")
