@@ -340,9 +340,10 @@ extern "C" int nrc_fism_grad(const float* c1, const float* q, const float* bias,
                              int32_t* touched_c1, int32_t* touched_item, int32_t stamp, float* loss, void* stream) {
     const int rc = fism_check(num_items, dim, pairwise, loss_kind, batch, alpha);
     if (rc) return rc;
-    NRC_REQUIRE(c1 && q && bias && hist_ptr && hist_idx && rows && num && items && third, NRC_E_VALUE,
+    // an empty batch launches nothing and may come without arrays, as in nrc_fism_query
+    NRC_REQUIRE(batch == 0 || (c1 && q && bias && hist_ptr && hist_idx && rows && num && items && third), NRC_E_VALUE,
                 "tables, the history CSR and the batch are required");
-    NRC_REQUIRE(!pairwise || num_neg, NRC_E_VALUE, "num_neg is required in the pairwise form");
+    NRC_REQUIRE(batch == 0 || !pairwise || num_neg, NRC_E_VALUE, "num_neg is required in the pairwise form");
     NRC_REQUIRE(grad_c1 && grad_q && grad_bias && touched_c1 && touched_item, NRC_E_VALUE,
                 "gradients and touched stamps are required");
     if (batch == 0) return NRC_OK;
@@ -382,9 +383,10 @@ extern "C" int nrc_fism_train_epoch(float* c1, float* q, float* bias, int32_t nu
     NRC_REQUIRE(opt_kind >= NRC_OPT_GD && opt_kind <= NRC_OPT_MOMENTUM, NRC_E_VALUE, "please select a suitable optimizer");
     NRC_REQUIRE(lr_t_host && hyper_host && slot0 && slot1 && step_loss, NRC_E_VALUE,
                 "lr_t_host, hyper_host, slot0, slot1 (the three variables' slots) and step_loss are required");
-    NRC_REQUIRE(c1 && q && bias && hist_ptr && hist_idx && rows && num && items && third, NRC_E_VALUE,
+    // an empty epoch may come without arrays: seq_epoch_loop runs no gradient step and no optimizer pass at n = 0
+    NRC_REQUIRE(n == 0 || (c1 && q && bias && hist_ptr && hist_idx && rows && num && items && third), NRC_E_VALUE,
                 "tables, the history CSR and the samples are required");
-    NRC_REQUIRE(!pairwise || num_neg, NRC_E_VALUE, "num_neg is required in the pairwise form");
+    NRC_REQUIRE(n == 0 || !pairwise || num_neg, NRC_E_VALUE, "num_neg is required in the pairwise form");
     NRC_REQUIRE(grad_c1 && grad_q && grad_bias && touched_c1 && touched_item, NRC_E_VALUE,
                 "gradients and touched stamps are required");
     const size_t tsz = pairwise ? sizeof(int32_t) : sizeof(float);
