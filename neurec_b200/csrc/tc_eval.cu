@@ -542,7 +542,7 @@ static size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
 // The bf16 copy + max row norm are reused across calls while the caller vouches that the table has
 // not changed: nrc_eval_tc_items_version(v != 0) keys the cache on (pointer, shape, v); version 0
 // (default) converts on every call.
-static int g_ch_pref = -1;      // filter threads per user: 1 (default) or 2 (nrc_eval_tc_epilogue_warps / NRC_TC_CH)
+static int g_ch_pref = 1;       // filter threads per user: 1 (default) or 2 (nrc_eval_tc_epilogue_warps)
 static int g_force_segments = 0;   // item segments per pass: 0 = heuristic, g >= 1 = min(g, tiles) (nrc_eval_tc_force_segments)
 static uint64_t g_items_version = 0, g_cached_version = 0;
 static const float* g_cached_ptr = nullptr;
@@ -576,7 +576,6 @@ int run_pass(int pass, const float* U, const int32_t* users, int num_rows, const
     const int row_tiles = (num_rows + kMU - 1) / kMU;
     // Tile width: 128 items (wgmma N) while two stages of them fit beside the staged scores; 64 for dim 192.
     const int lstride = (LQ <= 32) ? 33 : 65;
-    if (g_ch_pref < 0) { const char* e = getenv("NRC_TC_CH"); g_ch_pref = e ? atoi(e) : 1; }
     const int CH = (g_ch_pref == 2 && pass == 0) ? 2 : 1;   // the replay pass needs lists in ascending item order
     const int kNT = (D <= 128) ? 128 : 64;
     const size_t fixed = (kNT == 128 ? cand_smem_bytes<128>(D, 0, CH, lstride) : cand_smem_bytes<64>(D, 0, CH, lstride));
