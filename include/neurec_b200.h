@@ -52,6 +52,13 @@ extern "C" {
 #define NRC_OPT_RMSPROP 3
 #define NRC_OPT_MOMENTUM 4
 
+/* ItemKNN similarity transforms, model/general_recommender/ItemKNN.py:146-181, 476-500 (see nrc_itemknn_similarity) */
+#define NRC_ITEMKNN_NORM 0       /* cosine, adjusted, pearson, asymmetric */
+#define NRC_ITEMKNN_TANIMOTO 1   /* jaccard, tanimoto */
+#define NRC_ITEMKNN_DICE 2
+#define NRC_ITEMKNN_TVERSKY 3
+#define NRC_ITEMKNN_EUCLIDEAN 4
+
 int nrc_version(void);
 const char* nrc_last_error(void);
 
@@ -1230,6 +1237,59 @@ int nrc_fism_scores(const float* query, const float* q, const float* bias, int32
  *   gridDim.x (CTAs of 64 threads, a warp per sample or row; the score kernel: groups of 8 rows); +4 gridDim.y (the
  *   score kernel: item tiles of 256); +5 1 when the grid was capped above 64 * SMs samples or rows, else 0. */
 int nrc_fism_last_routes(int32_t* out);
+
+/* ======================================================================================
+ * ItemKNN (model/general_recommender/ItemKNN.py): item-item similarity, top-K neighbours, ratings = R . W
+ * ==================================================================================== */
+
+/* Bytes of the `work` buffer nrc_itemknn_similarity needs for num_items items: 0 while a CTA's row of num_items x 8 B
+ * fits in shared memory (220 KB), else one such row per CTA of the capped grid (4 * SMs CTAs). */
+int64_t nrc_itemknn_work_bytes(int32_t num_items);
+
+/* Compute_Similarity(...).compute_similarity(), ItemKNN.py:11-547, as ItemKNN.build_graph calls it (normalize=True).
+ * X [num_users, num_items] comes twice, as a CSR (csr_ptr i64 [U + 1], csr_idx i32, csr_val f64) and as its CSC
+ * (csc_ptr i64 [I + 1], csc_idx i32 users ascending, csc_val f64), values already centred (adjusted: minus the row
+ * average; pearson: minus the column average) or made binary (tanimoto, dice, tversky) by the caller.  va, vb f64 [I]
+ * are the per-item vectors the reference computes with numpy: NORM va = vb = sqrt(sum of squares), or (asymmetric)
+ * va = s^(2 alpha), vb = s^(2 (1 - alpha)); TANIMOTO / DICE / TVERSKY va = the sum of squares (vb unused);
+ * EUCLIDEAN va = the sum of squares, vb = its sqrt.  For column c, w_k = sum over users ascending of X[u,k] X[u,c],
+ * w_c = 0, then in the reference's order with correctly rounded f64 operations:
+ *   NORM       w * (1 / (va_c * vb_k + shrink + 1e-6))
+ *   TANIMOTO   w * (1 / (va_c + va_k - w + shrink + 1e-6))
+ *   DICE       w * (1 / (va_c + va_k + shrink + 1e-6))
+ *   TVERSKY    w * (1 / (w + (va_c - w) * tversky_alpha + (va_k - w) * tversky_beta + shrink + 1e-6))
+ *   EUCLIDEAN  1 / (sqrt((va_k + va_c - 2 w) / (vb_c * vb_k)) + shrink + 1e-9), and 0 at k = c.
+ * The top min(neighbor, I) values of the column by (value descending, row ascending, NaN last) are selected and those
+ * != 0.0 kept (the row-ascending tie rule is the one deviation: numpy's introselect orders ties its own way).  W is
+ * written in padded CSC form, slot-major: column c holds counts[c] entries, entry t at [t * I + c] of rows i32 and vals
+ * f32 (the float64 value rounded once), rows ascending; both arrays hold min(neighbor, I) * I entries.  integral != 0
+ * vouches that every value is an integer; with gram_bound (an upper bound on every |w_k|) at most 2^31 - 1 the dots
+ * are summed as int32, otherwise as f64.  work: nrc_itemknn_work_bytes(num_items) bytes (NULL when 0).  NRC_E_VALUE
+ * when num_users < 0, num_items < 1, kind is outside [0, 4], neighbor < 1, shrink or a tversky coefficient is NaN,
+ * an array is NULL or work is too small.  A rejected call writes nothing. */
+int nrc_itemknn_similarity(int32_t num_users, int32_t num_items, const int64_t* csr_ptr, const int32_t* csr_idx,
+                           const double* csr_val, const int64_t* csc_ptr, const int32_t* csc_idx,
+                           const double* csc_val, int32_t kind, const double* va, const double* vb, double shrink,
+                           double tversky_alpha, double tversky_beta, int32_t neighbor, int32_t integral,
+                           double gram_bound, void* work, int64_t work_bytes, int32_t* counts, int32_t* rows,
+                           float* vals, void* stream);
+
+/* ItemKNN.predict(users, None), ItemKNN.py:573 and 583-585: out f32 [batch, I], out[b, j] = the f64 sum over column
+ * j's entries k of W (ascending) with X[u, k] stored of X[u, k] * W[k, j], u = users[b], rounded once to f32: the
+ * order in which scipy's csr_matmat forms train.tocsc().dot(W).  The CSR is X's (the un-centred train values); W is
+ * nrc_itemknn_similarity's output at the same neighbor.  NRC_E_LIMIT when num_items is above 220 KB / 8 B * 32;
+ * NRC_E_VALUE when num_items < 1, neighbor < 1, batch < 0 or an array is NULL. */
+int nrc_itemknn_scores(int32_t num_items, const int64_t* csr_ptr, const int32_t* csr_idx, const double* csr_val,
+                       int32_t neighbor, const int32_t* counts, const int32_t* rows, const float* vals,
+                       const int32_t* users, int64_t batch, float* out, void* stream);
+
+/* Test hook of the ItemKNN kernels, as nrc_seq_last_routes: out i32[2 * 6], group k at out[6 * k].
+ *   groups: [0] the similarity kernel, [1] the score kernel.
+ *   fields: +0 0 the int32 accumulator, 1 the f64 one (similarity); +1 the tier: 0 the CTA's row in shared memory,
+ *   1 an int32 accumulator in shared memory and the keys in global work, 2 both in global work (similarity); +2
+ *   gridDim.x (a CTA per column / per user, grid-strided); +3 1 when that grid was capped (above 4 * SMs columns,
+ *   8 * SMs users), else 0; +4 min(neighbor, I); +5 dynamic shared memory in bytes. */
+int nrc_itemknn_last_routes(int32_t* out);
 
 /* Test hook of the sequential kernels (it reports and changes nothing; every route is chosen by the shape).
  * nrc_seq_last_routes: HOST bookkeeping of the most recent launch of each kernel group, written when a call launches

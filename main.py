@@ -30,7 +30,7 @@ def resolve_model(recommender):
             return getattr(importlib.import_module(name), recommender)
     raise ImportError("recommender '%s' is outside the accelerated hot path "
                       "(available: MF, MLP, NeuMF, LightGCN, NGCF, APR, SpectralCF, WRMF, SBPR, FPMC, TransRec, "
-                      "HRM, NPE, FPMCplus, Caser, FISM)" % recommender)
+                      "HRM, NPE, FPMCplus, Caser, FISM, ItemKNN)" % recommender)
 
 
 if __name__ == "__main__":

@@ -1281,6 +1281,87 @@ def fism_last_routes():
     return {k: dict(zip(FISM_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(FISM_KERNELS)}
 
 
+# ------------------------------------------------------------------------- ItemKNN: neighbourhood similarity
+ITEMKNN_KINDS = {"norm": 0, "tanimoto": 1, "dice": 2, "tversky": 3, "euclidean": 4}
+
+
+def itemknn_similarity(csr_ptr, csr_idx, csr_val, csc_ptr, csc_idx, csc_val, num_items, kind, va, vb, shrink,
+                       tversky_alpha, tversky_beta, neighbor, integral=None, gram_bound=None):
+    """Compute_Similarity(...).compute_similarity() (ItemKNN.py:11-547) on the device: W in padded CSC form,
+    (counts i32 [I], rows i32 [Kc, I], vals f32 [Kc, I]) with Kc = min(neighbor, I) and column c's entries at
+    [:counts[c], c], rows ascending.  X comes as its CSR and its CSC (f64 values, already centred or made binary);
+    va, vb f64 [I] are the per-item vectors (see nrc_itemknn_similarity); kind is a key of ITEMKNN_KINDS.
+    integral / gram_bound default to what the values show: integral when every value is an integer, the bound
+    max|x|^2 * (the longest column)."""
+    for t, name in ((csr_ptr, "csr_ptr"), (csc_ptr, "csc_ptr")):
+        _req(t, torch.int64, name)
+    for t, name in ((csr_idx, "csr_idx"), (csc_idx, "csc_idx")):
+        _req(t, torch.int32, name)
+    for t, name in ((csr_val, "csr_val"), (csc_val, "csc_val"), (va, "va"), (vb, "vb")):
+        _req(t, torch.float64, name)
+    ni = int(num_items)
+    if kind not in ITEMKNN_KINDS:
+        raise ValueError("similarity kind '%s' is not one of %s" % (kind, sorted(ITEMKNN_KINDS)))
+    if ni < 1 or int(neighbor) < 1:
+        raise ValueError("num_items >= 1 and neighbor >= 1 required")
+    if csc_ptr.numel() != ni + 1 or va.numel() != ni or vb.numel() != ni:
+        raise ValueError("csc_ptr must hold num_items + 1 entries and va, vb num_items")
+    if csr_idx.numel() != csc_idx.numel() or csr_val.numel() != csr_idx.numel() or csc_val.numel() != csc_idx.numel():
+        raise ValueError("the CSR and the CSC must hold the same entries")
+    if integral is None:
+        integral = bool(csr_val.numel() == 0 or torch.equal(csr_val, torch.round(csr_val)))
+    if gram_bound is None:
+        top = float(csr_val.abs().max()) if csr_val.numel() else 0.0
+        longest = int((csc_ptr[1:] - csc_ptr[:-1]).max()) if ni else 0
+        gram_bound = top * top * longest
+    kc = min(int(neighbor), ni)
+    dev = csr_val.device
+    counts = torch.empty(ni, dtype=torch.int32, device=dev)
+    rows = torch.empty((kc, ni), dtype=torch.int32, device=dev)
+    vals = torch.empty((kc, ni), dtype=torch.float32, device=dev)
+    L = _lib.load()
+    nbytes = int(L.nrc_itemknn_work_bytes(ni))
+    work = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev) if nbytes else None
+    check(L.nrc_itemknn_similarity(
+        csr_ptr.numel() - 1, ni, _p(csr_ptr), _p(csr_idx), _p(csr_val), _p(csc_ptr), _p(csc_idx), _p(csc_val),
+        ITEMKNN_KINDS[kind], _p(va), _p(vb), float(shrink), float(tversky_alpha), float(tversky_beta), int(neighbor),
+        1 if integral else 0, float(gram_bound), _p(work), nbytes, _p(counts), _p(rows), _p(vals), _stream()))
+    _count()
+    return counts, rows, vals
+
+
+def itemknn_scores(csr_ptr, csr_idx, csr_val, W, users):
+    """ItemKNN.predict(users, None) (ItemKNN.py:573, 583-585) on the device: f32 [len(users), I], the f64 sum of
+    X[u, k] * W[k, j] over column j's entries in ascending k (scipy's order for train.tocsc().dot(W)) rounded once.
+    W = (counts, rows, vals) from itemknn_similarity; X is the un-centred train CSR (f64 values)."""
+    _req(csr_ptr, torch.int64, "csr_ptr"); _req(csr_idx, torch.int32, "csr_idx"); _req(csr_val, torch.float64, "csr_val")
+    counts, rows, vals = W
+    _req(counts, torch.int32, "counts"); _req(rows, torch.int32, "rows"); _req(vals, torch.float32, "vals")
+    _req(users, torch.int32, "users")
+    ni = counts.numel()
+    if rows.dim() != 2 or rows.shape != vals.shape or rows.shape[1] != ni:
+        raise ValueError("W's rows and vals must be [min(neighbor, I), I]")
+    out = torch.empty((users.numel(), ni), dtype=torch.float32, device=users.device)
+    check(_lib.load().nrc_itemknn_scores(ni, _p(csr_ptr), _p(csr_idx), _p(csr_val), max(rows.shape[0], 1),
+                                         _p(counts), _p(rows), _p(vals), _p(users), users.numel(), _p(out),
+                                         _stream()))
+    _count()
+    return out
+
+
+ITEMKNN_KERNELS = ("similarity", "scores")
+ITEMKNN_ROUTE_FIELDS = ("acc", "tier", "grid", "capped", "k", "smem")
+
+
+def itemknn_last_routes():
+    """Routes of the most recent launch of each ItemKNN kernel (nrc_itemknn_last_routes) as {kernel: {field: value}};
+    -1 = no such launch yet or a field the kernel does not decide."""
+    nf = len(ITEMKNN_ROUTE_FIELDS)
+    out = (ctypes.c_int32 * (len(ITEMKNN_KERNELS) * nf))()
+    check(_lib.load().nrc_itemknn_last_routes(out))
+    return {k: dict(zip(ITEMKNN_ROUTE_FIELDS, out[i * nf:(i + 1) * nf])) for i, k in enumerate(ITEMKNN_KERNELS)}
+
+
 SEQ_KERNELS = ("fpmc_grad", "transrec_grad", "hrm_grad", "npe_grad", "fpmc_scores", "transrec_scores", "hrm_query",
                "npe_query", "npe_relu")
 SEQ_ROUTE_FIELDS = ("pairwise", "session_max", "pre_max", "grid_x", "grid_y", "capped", "window")
